@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Benchmark of the SelfRecon hot path on B200 (BASELINE.json metric, config[1]).
+"""Benchmark of the SelfRecon hot path on H100 (BASELINE.json metric, config[1]).
 
 One "step" = one pass of the hot path over one synthetic 512x512 frame:
   ray part : OptimizeSurfacePs (training thresholds: dthr 5e-5, 0.5 px angle, times=10) on every
@@ -9,7 +9,9 @@ One "step" = one pass of the hot path over one synthetic 512x512 frame:
 Inputs are resident in HBM for `value`; `e2e` repeats the step through the reference-facing
 drop-in API with pinned host buffers, H2D/D2H inside the timed region.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
+--dump-outputs writes what the last timed step computed (ray part and MC part) as DIR/<name>.npy; the inputs
+are seeded, so two builds can be compared output for output.
 Under torchrun (N>1) every rank renders its own frame (weak scaling, no data-path collective).
 """
 import argparse
@@ -37,11 +39,12 @@ def peaks():
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], tensor=d["bf16_tflops"], tensor_sustained=d.get("bf16_tflops_sustained"),
                     src="measured")
-    return dict(hbm=6650.0, tensor=1590.0, tensor_sustained=1400.0, src="fallback")
+    # NVIDIA's H100 SXM data sheet (700 W card): HBM3 bandwidth, dense BF16 -- ceilings, not measured rates
+    return dict(hbm=3350.0, tensor=989.0, tensor_sustained=None, src="H100 SXM data sheet")
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index):
         self.rows = []
@@ -155,8 +158,8 @@ def mc_part(sc, eng):
 
 def layer_roofline(dev, M, launches=24):
     """Live timing of the dominant kernel: one 512x512 softplus layer of the tracer on M rows
-    (tc_layer_pair_kernel), CUDA events on the launching stream, rotating operand buffers so that no
-    launch finds its rows in L2 (4 x (in + out) > 126 MB).  Bias and outputs are allocated once: the
+    (tc_sweep_kernel, one step), CUDA events on the launching stream, rotating operand buffers so that no
+    launch finds its rows in L2 (4 x (in + out) > 50 MB).  Bias and outputs are allocated once: the
     timed region holds nothing but the layer launches."""
     import ctypes as C
     from selfreconcode_b200 import ops, _lib
@@ -636,6 +639,26 @@ def run_reference(args, rank, world):
     print(json.dumps(line), flush=True)
 
 
+def dump_outputs(path, ray, grid, verts, faces, max_bytes=64 << 20):
+    """The last timed step's results as DIR/<name>.npy: the ray part's surface points, convergence mask and colours,
+    the MC mesh, and a fixed seeded sample (2^20 voxels, the same indices every run) of the 257^3 SDF grid, which
+    alone would exceed the 64 MB budget.  Integers are stored as float64 (exact), everything else as float32."""
+    os.makedirs(path, exist_ok=True)
+    pts, conv, rgb = ray
+    g = grid.reshape(-1)
+    idx = np.sort(np.random.default_rng(0).choice(g.numel(), size=min(g.numel(), 1 << 20), replace=False))
+    arrays = {"ray_points": pts, "ray_converged": conv, "ray_rgb": rgb, "mc_vertices": verts, "mc_faces": faces,
+              "sdf_grid_sample": g[torch.from_numpy(idx).to(g.device)], "sdf_grid_sample_index": idx}
+    out = {}
+    for name, t in arrays.items():
+        a = t.detach().cpu().numpy() if torch.is_tensor(t) else np.asarray(t)
+        out[name] = a.astype(np.float64 if np.issubdtype(a.dtype, np.integer) or a.dtype == np.float64 else np.float32)
+    total = sum(a.nbytes for a in out.values())
+    assert total <= max_bytes, "outputs of %d bytes exceed the %d-byte budget" % (total, max_bytes)
+    for name, a in out.items():
+        np.save(os.path.join(path, name + ".npy"), a)
+
+
 # --------------------------------------------------------------------------------------------------
 def main():
     ap = argparse.ArgumentParser()
@@ -645,6 +668,8 @@ def main():
     ap.add_argument("--impl", default="ours")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-train", action="store_true", help="skip the training-step section")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float32 / float64, <= 64 MB)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -668,7 +693,7 @@ def main():
     n_rays = R["rays"].shape[0]
     rays_d, init_d, bi_d = R["rays"].to(dev), R["init_pts"].to(dev), R["batch_inds"].to(dev)
     rays_h, init_h, bi_h = R["rays"].pin_memory(), R["init_pts"].pin_memory(), R["batch_inds"].pin_memory()
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 50 MB L2
 
     def barrier():
         if dist is not None:
@@ -691,7 +716,7 @@ def main():
             flush.zero_()
             e0, e1, e2, e3 = ev(), ev(), ev(), ev()
             e0.record()
-            ray_part(sc, rays_d, init_d, bi_d, stats)
+            ray_out = ray_part(sc, rays_d, init_d, bi_d, stats)
             e1.record()
             flush.zero_()
             e2.record()
@@ -703,6 +728,8 @@ def main():
         barrier()
         t_wall = time.perf_counter() - t_wall0
     launches = ops.LAUNCHES
+    if args.dump_outputs and rank == 0 and args.steps > 0:
+        dump_outputs(args.dump_outputs, ray_out, grid, v, f)
     # second number: weights change every step (a training loop): weight-norm fold + tensor-core weight packing
     # + an eager (not graph-replayed) trace are inside the timed region
     refold_ms = []
@@ -772,7 +799,7 @@ def main():
 
     train = None
     if not args.no_train:
-        train = train_part(sc, dev, rank, world, dist, max(2, min(args.steps, 10)), args.warmup)
+        train = train_part(sc, dev, rank, world, dist, args.steps, args.warmup)
         train_launches = ops.LAUNCHES
         # the scene's parameters moved (Adam): nothing below depends on their values
 
@@ -808,14 +835,12 @@ def main():
         "e2e": {"value": total_rays / (e2e_t * 1e-3), "unit": "rays/s", "h2d_bytes_per_step": int(h2d),
                 "d2h_bytes_per_step": int(d2h), "ms": e2e_t},
         "gpu_launches": int(launches),
-        "roofline": {"kernel": "tc_layer_pair_kernel<softplus,1> (tcgen05 cta_group::2 split-BF16 GEMM layer 512x512 of "
-                               "the tracer, M = rays of the frame; ~300 such launches per trace)",
+        "roofline": {"kernel": "tc_sweep_kernel<softplus,1> (wgmma split-BF16 GEMM layer 512x512 of "
+                               "the tracer, M = rays of the frame)",
                      "bound": "tensor", "achieved": layer_tf, "peak": pk["tensor"], "unit": "TFLOP/s",
                      "frac": layer_tf / pk["tensor"],
-                     # dram__bytes_read.sum + dram__bytes_write.sum of one launch at M = 50 333 from the
-                     # ncu --set full capture in profiles/r01c_summary.md (algorithmic: 103 MB in + 103 MB out)
-                     "traffic": 159.3e6 if n_rays == 50333 else None,
-                     "peak_source": pk["src"] + " bf16 cuBLAS burst", "ms_per_launch": layer_ms,
+                     "traffic": None,
+                     "peak_source": pk["src"], "ms_per_launch": layer_ms,
                      "mma_terms": 3, "tensor_pipe_frac": 3.0 * layer_tf / pk["tensor"],
                      "note": "achieved = algorithmic fp32 FLOPs of one layer launch (2*M*512*512, SURVEY 8d: 0.524 "
                              "MFLOP per point per hidden layer) / its average duration, CUDA events over %d "
@@ -831,8 +856,7 @@ def main():
         "roofline_mc": {"kernel": "mc_sign+mc_classify+mc_scan+mc_emit", "bound": "hbm",
                         "achieved": mc_bytes / mc_s / 1e9, "peak": pk["hbm"], "unit": "GB/s",
                         "frac": mc_bytes / mc_s / 1e9 / pk["hbm"],
-                        # ncu capture of the four kernels (profiles/r01c_summary.md); algorithmic = mc_bytes
-                        "traffic": 92.6e6 if GRID_N == 257 else None, "algorithmic_bytes": mc_bytes,
+                        "traffic": None, "algorithmic_bytes": mc_bytes,
                         "ms": mc_s * 1e3,
                         "peak_source": pk["src"]},
         "clocks": clk.summary(),
@@ -841,12 +865,12 @@ def main():
     if train is not None:
         wg_ms, wg_flops = wgrad_roofline(dev)
         wg_tf = wg_flops / (wg_ms * 1e-3) / 1e12
-        train["gpu_launches_own_kernels_per_step"] = int(train_launches // max(2, min(args.steps, 10)))
-        train["roofline"] = {"kernel": "tc_wgrad_kernel (tcgen05 MN-major split-BF16 GEMM dW = delta^T x, 512x512 over "
+        train["gpu_launches_own_kernels_per_step"] = int(train_launches // max(1, args.steps))
+        train["roofline"] = {"kernel": "tc_wgrad_kernel (wgmma MN-major split-BF16 GEMM dW = delta^T x, 512x512 over "
                                        "393 216 rows: the def_regu block's translator layers)", "bound": "tensor",
                              "achieved": wg_tf, "peak": pk["tensor"], "unit": "TFLOP/s", "frac": wg_tf / pk["tensor"],
                              "ms_per_launch": wg_ms, "mma_terms": 3, "tensor_pipe_frac": 3.0 * wg_tf / pk["tensor"],
-                             "traffic": None, "peak_source": pk["src"] + " bf16 cuBLAS burst"}
+                             "traffic": None, "peak_source": pk["src"]}
         line["train"] = train
     if not args.no_cpu_baseline and world == 1:
         threads = pick_threads()

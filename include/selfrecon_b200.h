@@ -1,5 +1,5 @@
 /*
- * selfrecon_b200.h -- C ABI of libselfrecon_b200.so (B200 / sm_100a).
+ * selfrecon_b200.h -- C ABI of libselfrecon_b200.so (H100 / sm_90a).
  *
  * This is the drop-in boundary for the SelfRecon per-frame optimisation hot path
  * (SURVEY.md section 8).  Every entry point takes plain device pointers, sizes and a
@@ -255,16 +255,14 @@ int sr_shade_geometry(const sr_mlp_desc* sdf, const sr_mlp_desc* dnet, const sr_
                       float* feat, int nfeat, float* dpos, uint8_t* inv_ok, cudaStream_t s);
 
 /* ------------------------------------------------------------------------------------------
- * Tensor-core engine for the dense layers (tcgen05 + TMEM + TMA bulk copies): split-BF16 GEMM
- * (x = b1 + b2, three bf16 MMAs per product, fp32 accumulation in TMEM; measured error of the
- * 8x512 SDF vs fp64: 2.4e-5 abs), one launch per layer,  C = act(A * W^T + b)  with the epilogue
- * (bias, activation, forward-mode tangent scaling, skip concat, re-split) fused; layers whose
- * width is a multiple of 256 run on CTA pairs (cta_group::2).  Operands are kept in
- * global memory in the UMMA canonical tile layout (see csrc/tc_gemm.cu):
+ * Tensor-core engine for the dense layers (Hopper wgmma + TMA bulk copies): split-BF16 GEMM
+ * (x = b1 + b2, three bf16 MMAs per product, fp32 accumulation in registers), one launch per
+ * layer,  C = act(A * W^T + b)  with the epilogue (bias, activation, forward-mode tangent scaling,
+ * skip concat, re-split) fused.  Operands are kept in global memory in the canonical no-swizzle
+ * tile layout of the wgmma descriptors (see csrc/tc_gemm.cu):
  *   sr_tc_act_bytes(M,K) / sr_tc_weight_bytes(N,K): buffer sizes of tiled activations / weights
  *   sr_tc_pack_rows    : fp32 row-major [M][K] (ld) -> tiled split-bf16 activations
  *   sr_tc_pack_weights : fp32 row-major [N][K] (ld) effective weights -> tiled split-bf16
- *                        (the single-CTA layout followed by the CTA-pair layout)
  *   sr_tc_linear       : one layer. A (tiled, K), W (tiled, N x K), bias [pad256(N)];
  *                        n_valid output columns; ch = rows per point (1, or 4 = value + 3
  *                        tangents: tangent rows get act'(z_value) * acc, no bias);
@@ -317,7 +315,7 @@ typedef struct sr_tc_step {
   float scale, mul_scale;
 } sr_tc_step;
 
-/* sr_tc_sweep: L <= 12 chained steps (step l+1 reads the tiles step l wrote) in ONE launch: a CTA pair keeps its
+/* sr_tc_sweep: L <= 12 chained steps (step l+1 reads the tiles step l wrote) in ONE launch: a CTA keeps its
  * row tiles through all steps, the only inter-step dependency is inside a CTA (network.py:66-83 ImplicitNetwork.forward
  * layer loop; its reverse for the tracer's gradient, FindSurfacePs.py:128-140).  Same results as L sr_tc_linear calls.
  * Restrictions: activations NONE / SOFTPLUS100 / RELU; a buffer must not be used with two different tile widths
@@ -343,7 +341,7 @@ int sr_raster_mesh(const float* verts_screen, const int64_t* faces, int64_t N, i
  * ch == 4 it propagates the cotangents of forward-mode rows (value + 3 tangents per point), i.e. second order.
  *   sr_tc_wgrad   dW[N x K] (row-major, ld) = delta^T x over M rows; delta / x = tiled split-bf16 activations with
  *                 Kd / Kx feature columns (each a multiple of 32); `part` = scratch of
- *                 sr_tc_wgrad_partial_bytes(M, Kd, Kx, NULL) bytes.  tcgen05 with MN-major operands: no transposes.
+ *                 sr_tc_wgrad_partial_bytes(M, Kd, Kx, NULL) bytes.  wgmma with MN-major operands: no transposes.
  *   sr_tc_colsum  partial[slice][k] = sum over rows with row % ch == 0 (value rows) of the tiled activations: the
  *                 bias gradient after a sum over slices.
  *   sr_tc_unpack_rows   tiled split-bf16 -> fp32 [M][K] (inverse of sr_tc_pack_rows).                           */
@@ -410,8 +408,8 @@ int sr_band_select(const float* values, int64_t n, float center, float eps, int3
                    int32_t* counter, cudaStream_t s);
 int sr_sdf_forward_indexed(const sr_mlp_desc* net, const float* pts, int64_t P, const int32_t* index,
                            const int32_t* m_dev, float* sdf, cudaStream_t s);
-/* Same contract for the first `cap` entries of the list, as one column-split launch per layer (fp32 FMAs): ~0.1 ms for
- * a short list where the persistent engine's per-tile latency is ~1 ms.  work = sr_sdf_small_work_bytes(cap) bytes. */
+/* Same contract for the first `cap` entries of the list, as one column-split launch per layer (fp32 FMAs): short lists
+ * do not pay the persistent engine's per-tile latency.  work = sr_sdf_small_work_bytes(cap) bytes. */
 int64_t sr_sdf_small_work_bytes(int cap);
 int sr_sdf_forward_small(const sr_mlp_desc* net, const float* pts, int64_t P, const int32_t* index,
                          const int32_t* m_dev, float* sdf, void* work, int cap, cudaStream_t s);

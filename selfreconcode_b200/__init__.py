@@ -1,4 +1,4 @@
-"""selfrecon-b200: B200-native (sm_100a) implementation of SelfRecon's per-frame hot path.
+"""selfrecon-b200: H100-native (sm_90a) implementation of SelfRecon's per-frame hot path.
 
 Layout
   csrc/        CUDA kernels + the C ABI (include/selfrecon_b200.h) -> lib/libselfrecon_b200.so

@@ -1,11 +1,11 @@
-// Shared device/host helpers for the selfrecon-b200 kernels (sm_100a only).
+// Shared device/host helpers for the selfrecon-b200 kernels (sm_90a: H100).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 
 #include "../../include/selfrecon_b200.h"
 
-#define SR_NUM_SMS_B200 148
+#define SR_NUM_SMS 132   // H100 SXM
 
 // Launch-error -> C-ABI return code. Never synchronises.
 static inline int sr_launch_status() {
@@ -22,7 +22,7 @@ static inline int sr_div_up(long long a, long long b) { return (int)((a + b - 1)
 // Grid sized as a multiple of the SM count (persistent / grid-stride kernels).
 static inline int sr_grid_for(long long n, int threads, int ctas_per_sm) {
   long long need = (n + threads - 1) / threads;
-  long long cap = (long long)SR_NUM_SMS_B200 * ctas_per_sm;
+  long long cap = (long long)SR_NUM_SMS * ctas_per_sm;
   if (need < 1) need = 1;
   return (int)(need < cap ? need : cap);
 }

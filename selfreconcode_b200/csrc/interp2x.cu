@@ -7,7 +7,7 @@
 // by a power of two) and is a boundary voxel iff those sources disagree on `v > balance`.
 //
 // HBM-bound: 5 B written per output voxel, sources come from L1/L2.  One thread per output
-// voxel along x (coalesced 4 B + 1 B stores), grid = multiple of 148 SMs, grid-stride.
+// voxel along x (coalesced 4 B + 1 B stores), grid = multiple of the SM count, grid-stride.
 #include "common.cuh"
 
 namespace {

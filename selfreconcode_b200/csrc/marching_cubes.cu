@@ -211,8 +211,8 @@ __device__ __forceinline__ int load_cube(const float* __restrict__ sdf, int nx, 
 // Pass 2 (one THREAD per 32-cell word): the eight corner bit-words of the word's cells are the sign
 // words of rows (i,j) (i+1,j) (i+1,j+1) (i,j+1) and the same shifted by one k; crossed-edge flags are
 // XORs of whole words, active cells are where the eight words disagree, and only those cells (a few
-// per cent) index the triangle table.  The first version computed a cube index per lane from eight
-// float loads and was issue bound at 4 % of HBM (profiles/r01b_summary.md).
+// per cent) index the triangle table instead of building a cube index per lane from eight float loads
+// (an issue-bound loop).
 constexpr int kSignWordsPerWarp = 8;
 __global__ void __launch_bounds__(kThreads)
 mc_sign_kernel(const float* __restrict__ sdf, McLayout L, float iso) {

@@ -4,7 +4,7 @@
 //   inv = adj(m)/det ; if |det| < 1e-4 (compared in double) -> inv = 0, check = false
 //   backward: out = -(C^T G C^T) with C = inv.
 //
-// B200 notes: the op is a pure HBM stream (73 B / matrix forward, 108 B backward), so the
+// Notes: the op is a pure HBM stream (73 B / matrix forward, 108 B backward), so the
 // kernel stages each CTA's contiguous [256 x 9] block through shared memory to turn the
 // stride-9 per-thread accesses of the reference into fully coalesced 128-bit global
 // transactions; the grid is a multiple of the SM count with a grid-stride loop.

@@ -13,13 +13,13 @@
 // transposed weights, no second kernel.
 //
 // All arithmetic is fp32 (the ray finder's convergence test is |f| < 5e-5, SURVEY.md
-// section 7 "hard parts"); this FFMA engine is the accuracy reference for the tcgen05
-// 3xTF32 variant planned next (DESIGN.md).
+// section 7 "hard parts"); this FFMA engine is the accuracy reference for the split-BF16
+// tensor-core engine (tc_gemm.cu).
 #pragma once
 #include "common.cuh"
 
 #ifndef SR_GEMM_UNROLL
-#define SR_GEMM_UNROLL 8   // measured on B200: 2 / 4 / 8 within 2 %, 8 marginally best
+#define SR_GEMM_UNROLL 8
 #endif
 #ifndef SR_WARPS
 #define SR_WARPS 8        // 8: 8x16 thread tile, <=255 regs;  16: 8x8 thread tile, <=128 regs
@@ -202,8 +202,7 @@ __device__ __forceinline__ float softplus100(float z, float& deriv) {
   if (bz > 20.0f) { deriv = 1.0f; return z; }
 #if SR_FAST_ACT
   // MUFU.EX2 / MUFU.LG2 / fast divide: |error| <= ~3e-6 relative on e, i.e. < 3e-8 absolute on the
-  // activation (values are O(0.01..1)); the libm path costs ~3x the instructions per element
-  // and the epilogue was 15 % of all issued instructions (profiles/r01a_summary.md).
+  // activation (values are O(0.01..1)); the libm path costs ~3x the instructions per element.
   const float e = __expf(bz);
   deriv = __fdividef(e, e + 1.0f);
   return __logf(1.0f + e) * 0.01f;
@@ -252,8 +251,6 @@ __device__ __forceinline__ void layer_gemm(const Smem& s, Pipe& cp, Prod& prod, 
     sr_mbar_wait(&s.full[cp.slot], cp.phase);
     const float* wst = s.wring + (size_t)cp.slot * kStageFloats + 4 * lane + ch * 128;
     const float* ak = arow + (size_t)sl * kKT * kRowStride;
-    // (The "no_instruction" stalls seen in profiles/r01a_summary.md come from the epilogue code,
-    // not from this loop: unrolling 2 / 4 / 8 k-steps measured within 2 % of each other.)
 #pragma unroll kGemmUnroll
     for (int kk = 0; kk < kKT; ++kk) {
       const float4 a0 = *reinterpret_cast<const float4*>(ak + kk * kRowStride);

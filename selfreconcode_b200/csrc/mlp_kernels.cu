@@ -869,9 +869,9 @@ int validate_net(const sr_mlp_desc* net, int T) {
 // ---------------------------------------------------------------------------------------------
 // Small-batch fp32 evaluation of the SDF value for a LIST of points (sign / threshold decisions on the few values the
 // tensor-core engine leaves inside its error band).  The persistent engine above is throughput-shaped: one CTA walks
-// all layers of a 64-row tile, ~1 ms of latency however few points there are.  Here every layer is one launch whose
-// CTAs split the COLUMNS (64 per CTA) and a group of 8 listed points, so a handful of points uses the whole GPU:
-// 9 launches of ~10-20 us.  Plain fp32 FMAs in k order; activations fp32 in global scratch [cap][512] x 2.
+// all layers of a 64-row tile, the same latency however few points there are.  Here every layer is one launch whose
+// CTAs split the COLUMNS (64 per CTA) and a group of 8 listed points, so a handful of points uses the whole GPU
+// (9 short launches).  Plain fp32 FMAs in k order; activations fp32 in global scratch [cap][512] x 2.
 // ---------------------------------------------------------------------------------------------
 constexpr int kSmallPts = 8;     // listed points per CTA
 constexpr int kSmallCols = 64;   // output columns per CTA
@@ -993,7 +993,7 @@ int set_smem(K kernel) {
 }
 
 int grid_for_tiles(long long ntiles) {
-  return (int)(ntiles < SR_NUM_SMS_B200 ? (ntiles < 1 ? 1 : ntiles) : SR_NUM_SMS_B200);
+  return (int)(ntiles < SR_NUM_SMS ? (ntiles < 1 ? 1 : ntiles) : SR_NUM_SMS);
 }
 
 }  // namespace
@@ -1202,7 +1202,7 @@ int sr_trace_step(const sr_mlp_desc* sdf, const sr_mlp_desc* dnet, const sr_lbs_
 }
 
 int64_t sr_trace_scratch_bytes(void) {
-  return (int64_t)SR_NUM_SMS_B200 * (int64_t)kScratchPerCta * (int64_t)sizeof(float);
+  return (int64_t)SR_NUM_SMS * (int64_t)kScratchPerCta * (int64_t)sizeof(float);
 }
 
 int sr_trace_step_rev(const sr_mlp_desc* sdf, const sr_mlp_desc* dnet, const sr_lbs_params* lbs,
@@ -1273,5 +1273,5 @@ int sr_shade_geometry(const sr_mlp_desc* sdf, const sr_mlp_desc* dnet, const sr_
 }
 
 int sr_abi_version(void) { return 1; }
-const char* sr_build_info(void) { return "selfrecon_b200 sm_100a fp32-ffma-fused " __DATE__; }
+const char* sr_build_info(void) { return "selfrecon_b200 sm_90a fp32-ffma-fused " __DATE__; }
 }

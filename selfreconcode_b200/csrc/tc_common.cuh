@@ -1,5 +1,5 @@
 // Shared pieces of the tensor-core engine (tc_gemm.cu: layer GEMMs, tc_wgrad.cu: weight-gradient GEMMs):
-// tile geometry of the pre-tiled split-bf16 operands, tcgen05 / TMEM wrappers.
+// tile geometry of the pre-tiled split-bf16 operands, Hopper wgmma wrappers.
 #pragma once
 #include <cuda_bf16.h>
 
@@ -11,30 +11,12 @@ namespace sr_tc {
 #define SR_TC_PLANES 2
 #endif
 constexpr int kPlanes = SR_TC_PLANES;
-constexpr int BM = 128, BN = 256, BK = 32, STAGES = kPlanes == 2 ? 4 : 3;
-// Epilogue warps per CTA, per kernel family: the forward epilogues (bias, activation, re-split) are latency-bound with
-// two warps per scheduler and fit 96 registers, so they run 16 warps (four per TMEM lane quarter, 64 columns each:
-// measured -7 % per layer at M = 50 333); the reverse epilogues prefetch their operand tiles and need the 168-register
-// budget of 8 warps (at 16 they spill: +40 %).
-#ifndef SR_TC_EPI_WARPS_FWD
-#define SR_TC_EPI_WARPS_FWD 16
-#endif
-#ifndef SR_TC_EPI_WARPS_REV
-#define SR_TC_EPI_WARPS_REV 8
-#endif
-__host__ __device__ constexpr int epi_warps(bool mul) { return mul ? SR_TC_EPI_WARPS_REV : SR_TC_EPI_WARPS_FWD; }
-__host__ __device__ constexpr int epi_threads(bool mul) { return 64 + 32 * epi_warps(mul); }
-__host__ __device__ constexpr int epi_part_cols(int ew) { return 256 / (ew / 4); }     // accumulator columns per epilogue warp
-__host__ __device__ constexpr int epi_chunks(int ew) { return epi_part_cols(ew) / 32; }  // 32-column chunks per warp
-static_assert((SR_TC_EPI_WARPS_FWD == 8 || SR_TC_EPI_WARPS_FWD == 16) &&
-              (SR_TC_EPI_WARPS_REV == 8 || SR_TC_EPI_WARPS_REV == 16), "epilogue warps: 8 or 16");
-constexpr int kMaxEpiWarps = 16;
+constexpr int BM = 128, BN = 256, BK = 32, STAGES = kPlanes == 2 ? 3 : 2;
 constexpr int A_PLANE = BM * BK;          // elements
 constexpr int W_PLANE = BN * BK;
 constexpr int A_STAGE = kPlanes * A_PLANE;   // 2 planes: 16 KB
 constexpr int W_STAGE = kPlanes * W_PLANE;   // 2 planes: 32 KB
 constexpr uint32_t A_STAGE_BYTES = A_STAGE * 2, W_STAGE_BYTES = W_STAGE * 2;
-constexpr size_t kSmem = (size_t)STAGES * (A_STAGE_BYTES + W_STAGE_BYTES) + 256;
 
 // ---- tiled ("pre-swizzled") global layouts ----------------------------------------------------
 // A: [row tile mt][k chunk kc][plane p][k8 (4)][row group (16)][row (8)][elem (8)]
@@ -57,57 +39,61 @@ __device__ __forceinline__ void split3(float x, __nv_bfloat16& b1, __nv_bfloat16
   b3 = __float2bfloat16_rn(r2);
 }
 
-// ---- tcgen05 wrappers ------------------------------------------------------------------------
+// ---- wgmma wrappers (sm_90a) ------------------------------------------------------------------
+// Shared-memory matrix descriptor, no swizzle: start[0,14) lbo[16,30) sbo[32,46) (all >> 4).
+// LBO = byte stride between adjacent 8x8 core matrices along K, SBO = along M / N.
 __device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  // cute::UMMA::SmemDescriptor: start[0,14) lbo[16,30) sbo[32,46) version[46,48)=1, swizzle none
   uint64_t d = (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= (uint64_t)1 << 46;
   return d;
 }
-// kind::f16 instruction descriptor: D=f32, A=B=bf16, both K-major, M=128, N=256
-constexpr uint32_t kIdescBase = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BM >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// Named barrier over the 128 threads of one warpgroup (ids 1.. ; 0 is __syncthreads).
+__device__ __forceinline__ void warpgroup_sync(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
 
-__device__ __forceinline__ void mma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                         uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+#define SR_ACC8(c, d, i)                                                                                \
+  c(d[i]), c(d[i + 1]), c(d[i + 2]), c(d[i + 3]), c(d[i + 4]), c(d[i + 5]), c(d[i + 6]), c(d[i + 7])
+#define SR_ACC32(c, d, i) SR_ACC8(c, d, i), SR_ACC8(c, d, i + 8), SR_ACC8(c, d, i + 16), SR_ACC8(c, d, i + 24)
+#define SR_ACC128(c, d) SR_ACC32(c, d, 0), SR_ACC32(c, d, 32), SR_ACC32(c, d, 64), SR_ACC32(c, d, 96)
+#define SR_WGMMA_M64N256K16_BF16                                                                                   \
+  "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"                                                            \
+  "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "                                                         \
+  "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, "     \
+  "%23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, "      \
+  "%44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, "      \
+  "%65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, "      \
+  "%86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, "     \
+  "%106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, "   \
+  "%124, %125, %126, %127}, %128, %129, p, 1, 1, %131, %132;\n\t}\n"
+
+// D[64 x 256] (fp32, registers of the warpgroup) (+)= A[64 x 16] * B[16 x 256], both bf16 from shared memory.
+// TA / TB = 1: the operand is MN-major (transposed) in shared memory.  FIRST: D = A * B, the old accumulator is
+// neither read nor kept live (write-only register operands).  Fragment of thread t (warp w = t / 32 of the
+// warpgroup, lane l): d[4 i + {0, 1}] = row 16 w + l / 4, columns 8 i + 2 (l % 4) + {0, 1}; d[4 i + {2, 3}]: row + 8.
+#define SR_OUT(x) "=f"(x)
+#define SR_INOUT(x) "+f"(x)
+template <int TA, int TB, bool FIRST>
+__device__ __forceinline__ void wgmma_m64n256k16(float (&d)[128], uint64_t adesc, uint64_t bdesc) {
+  if constexpr (FIRST)
+    asm volatile(SR_WGMMA_M64N256K16_BF16
+                 : SR_ACC128(SR_OUT, d)
+                 : "l"(adesc), "l"(bdesc), "r"(0), "n"(TA), "n"(TB));
+  else
+    asm volatile(SR_WGMMA_M64N256K16_BF16
+                 : SR_ACC128(SR_INOUT, d)
+                 : "l"(adesc), "l"(bdesc), "r"(1), "n"(TA), "n"(TB));
 }
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   sr_smem_u32(bar))
-               : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-#define SR_TMEM_REGS32(v)                                                                          \
-  "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),  \
-  "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]),          \
-  "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]),        \
-  "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]),        \
-  "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-#define SR_TMEM_REGS32_RW(v)                                                                       \
-  "+r"(v[0]), "+r"(v[1]), "+r"(v[2]), "+r"(v[3]), "+r"(v[4]), "+r"(v[5]), "+r"(v[6]), "+r"(v[7]),  \
-  "+r"(v[8]), "+r"(v[9]), "+r"(v[10]), "+r"(v[11]), "+r"(v[12]), "+r"(v[13]), "+r"(v[14]),          \
-  "+r"(v[15]), "+r"(v[16]), "+r"(v[17]), "+r"(v[18]), "+r"(v[19]), "+r"(v[20]), "+r"(v[21]),        \
-  "+r"(v[22]), "+r"(v[23]), "+r"(v[24]), "+r"(v[25]), "+r"(v[26]), "+r"(v[27]), "+r"(v[28]),        \
-  "+r"(v[29]), "+r"(v[30]), "+r"(v[31])
-// asynchronous TMEM -> register load of 32 columns (this warp's 32 lanes); pair with tmem_wait
-__device__ __forceinline__ void tmem_ld32_async(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-      : SR_TMEM_REGS32(v)
-      : "r"(taddr));
-}
-// the registers are in/out operands so that no consumer can be scheduled above the wait
-__device__ __forceinline__ void tmem_wait(uint32_t (&v)[32]) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" : SR_TMEM_REGS32_RW(v)::"memory");
-}
+#undef SR_OUT
+#undef SR_INOUT
+#undef SR_WGMMA_M64N256K16_BF16
+#undef SR_ACC128
+#undef SR_ACC32
+#undef SR_ACC8
 
 }  // namespace sr_tc

@@ -1,28 +1,26 @@
-// Tensor-core engine for the dense layers: split-BF16 GEMM on tcgen05 with fp32 accumulation in TMEM
-// (SURVEY.md section 7 "hard parts": the ray finder tests |f| < 5e-5; a single BF16 or TF32 pass does
-// not hold that).  Every fp32 operand is split into bf16 planes x = b1 + b2 (+ b3) and the product is
+// Tensor-core engine for the dense layers: split-BF16 GEMM on Hopper wgmma with fp32 accumulation in
+// registers (SURVEY.md section 7 "hard parts": the ray finder tests |f| < 5e-5; a single BF16 or TF32 pass
+// does not hold that).  Every fp32 operand is split into bf16 planes x = b1 + b2 (+ b3) and the product is
 // assembled from the leading cross terms:
 //     2 planes / 3 MMAs (default):  x*w ~= b1w1 + b1w2 + b2w1         (dropped: <= 2^-16 relative)
 //     3 planes / 6 MMAs (-DSR_TC_PLANES=3): + b2w2 + b1w3 + b3w1      (dropped: <= 2^-24 relative)
-// Measured on B200 against an fp64 evaluation of the 8x512 SDF (tools/tc_terms.py): the tensor core
-// adds each MMA into the fp32 accumulator with truncation, so the error of a K=512 layer is dominated
-// by the NUMBER of accumulations (K/16 per term), not by the dropped terms -- 3 terms: max |err|
-// 2.4e-5, 6 terms: 3.4e-5 (FFMA engine: 2.3e-6; parity bar 1e-4).  Fewer terms are both faster
-// and closer, hence the default.
+// The tensor core adds each MMA into the fp32 accumulator with truncation, so the error of a K=512 layer is
+// dominated by the NUMBER of accumulations (K/16 per term) rather than by the dropped terms (tools/tc_terms.py
+// compares the two builds).
 //
-// One launch = one layer  C[M x N] = act(A[M x K] * W^T + b)  over all row tiles:
-//   * operands live in global memory already in the canonical (no-swizzle, K-major) shared
-//     memory layout of the UMMA descriptors -- 128-byte core matrices (8 rows x 8 bf16), tiles
-//     of 128 (or 256) rows x 32 k, the split planes of a tile contiguous -- so ONE TMA bulk
-//     copy (cp.async.bulk + mbarrier) per operand per stage lands a ready-to-use tile and no
-//     tensor map is needed.  The previous layer's epilogue writes its output directly in that
-//     layout (activations stay L2-resident between layers for the batch sizes used here);
-//   * warp-specialised, persistent CTAs: warp 0 = TMA producer, warp 1 = single-thread
-//     tcgen05.mma issuer (+ TMEM alloc), warps 2-9 = epilogue (tcgen05.ld -> bias, activation,
-//     forward-mode tangent scaling or reverse-mode act' multiply, re-split to bf16 planes, tiled
-//     store); the epilogue is specialised at compile time per (activation, rows-per-point, mode);
-//   * 4-stage shared-memory ring (48 KB per stage), two 256-column fp32 accumulators in TMEM so
-//     the epilogue of tile i overlaps the MMAs of tile i+1.
+// One launch runs one layer  C[M x N] = act(A[M x K] * W^T + b)  over all row tiles, or a whole sweep of layers:
+//   * operands live in global memory already in the canonical (no-swizzle, K-major) shared memory layout
+//     of the wgmma descriptors -- 128-byte core matrices (8 rows x 8 bf16), tiles of 128 (or 256) rows
+//     x 32 k, the split planes of a tile contiguous -- so ONE TMA bulk copy (cp.async.bulk + mbarrier)
+//     per operand per stage lands a ready-to-use tile and no tensor map is needed.  The previous layer's
+//     epilogue writes its output directly in that layout (activations stay L2-resident between layers
+//     for the batch sizes used here);
+//   * warp-specialised, persistent CTAs: warpgroup 0 = TMA producer, warpgroups 1-2 = wgmma on 64 rows
+//     each, then the epilogue of those rows (bias, activation, forward-mode tangent scaling or
+//     reverse-mode act' multiply, re-split to bf16 planes, tiled store); the epilogue is specialised at
+//     compile time per (activation, rows-per-point, mode);
+//   * 3-stage shared-memory ring (48 KB per stage): the bulk copies of the next tile run under the epilogue, the
+//     MMAs do not (both consumer warpgroups are in the epilogue of the same tile; DESIGN.md section 8).
 // The FFMA engine (mlp_kernels.cu) stays the accuracy reference; tests compare both.
 #include <cstdlib>
 
@@ -33,11 +31,11 @@ namespace sr_tc {
 struct LayerArgs {
   const __nv_bfloat16* A;   // tiled activations  [MT][KC][3][128x32]
   const __nv_bfloat16* W;   // tiled weights      [NT][KC][planes][256x32]
-  const __nv_bfloat16* Wp;  // the same weights in the CTA-pair layout [NT][KC][half][planes][128x32]
   const float* bias;        // [NT*256]
   long long M;              // valid rows
   int MT, NT, KC;           // row tiles, col tiles, k chunks (K = 32*KC)
-  int n_gemm;               // columns the GEMM produces (<= NT*256); the MMA N of the last tile shrinks to it
+  int n_gemm;               // columns the GEMM produces (<= NT*256); the MMAs always run N = 256 over zero-padded
+                            // weight rows, the epilogue skips the chunks past n_gemm
   int n;                    // valid output columns
   int ch;                   // rows per point: 1 (value only) or 4 (value + 3 tangents)
   // outputs (either may be null)
@@ -147,7 +145,7 @@ struct EpiRow {
 // zero padding / skip-connection columns of the next layer's input are produced).
 template <int ACT, int CH, bool MUL, bool PF = true>
 __device__ __forceinline__ void epi_chunk(const LayerArgs& a, const EpiRow& r, uint32_t (&v)[32], int chunk,
-                                          bool live, bool wait_v = false) {
+                                          bool live) {
   const int c0 = r.nt * BN + chunk * 32;
   float o[32];
   if (live) {
@@ -158,15 +156,12 @@ __device__ __forceinline__ void epi_chunk(const LayerArgs& a, const EpiRow& r, u
                                 (size_t)(r.row_in_tile >> 3) * 64 + (r.row_in_tile & 7) * 8;
       const float kk = -144.26950408889634f * a.mul_inv_scale;   // -100 log2(e) / scale
       // optional fp32 act'(z) of the previous layer's VALUE rows (written by its forward launch as `dstash`)
-      // rows past M read row 0's entries (discarded below): the predicate stays warp-uniform, so the warp is
-      // converged at the .aligned TMEM wait that follows the loads
+      // rows past M read row 0's entries (discarded below)
       const long long srow = r.row_ok ? (CH == 4 ? (r.row & ~3LL) : r.row) : 0;
       const float* stash = a.dstash == nullptr ? nullptr : a.dstash + (size_t)srow * r.ds_ld + c0;
       const bool use_stash = (ACT == SR_ACT_SOFTPLUS100) && stash != nullptr;
-      // all global operands of the chunk first (8 x 16 B of activation tiles, 8 x 16 B of stash): 16 loads in flight
-      // per thread -- with two epilogue warps per scheduler nothing else hides their latency
-      // (PF = false: the 16-warp build of the reverse kernels has 96 registers -- operands are requested per group of
-      //  8 columns and the extra warps hide the latency instead)
+      // PF: all global operands of the chunk first (8 x 16 B of activation tiles, 8 x 16 B of stash), 16 loads in
+      // flight per thread; PF = false requests them per group of 8 columns (fewer registers)
       uint4 q0[PF ? 4 : 1], q1[PF ? 4 : 1];
       float st[PF ? 32 : 1];
       if constexpr (PF) {
@@ -183,8 +178,6 @@ __device__ __forceinline__ void epi_chunk(const LayerArgs& a, const EpiRow& r, u
           }
         }
       }
-      __syncwarp();
-      if (wait_v) tmem_wait(v);     // the accumulator chunk was requested by the caller before this function
 #pragma unroll
       for (int g = 0; g < 4; ++g) {
         uint4 a0, a1;
@@ -249,7 +242,6 @@ __device__ __forceinline__ void epi_chunk(const LayerArgs& a, const EpiRow& r, u
         }
       }
     } else {
-      if (wait_v) tmem_wait(v);
 #pragma unroll
       for (int j4 = 0; j4 < 8; ++j4) {
         const float4 b4 = __ldg(reinterpret_cast<const float4*>(a.bias + c0) + j4);
@@ -323,456 +315,33 @@ __device__ __forceinline__ void epi_chunk(const LayerArgs& a, const EpiRow& r, u
   }
 }
 
-template <int ACT, int CH, bool MUL>
-__global__ void __launch_bounds__(epi_threads(MUL), 1) tc_layer_kernel(const __grid_constant__ LayerArgs a) {
-  constexpr int kEpiWarps = epi_warps(MUL), kPartCols = epi_part_cols(kEpiWarps), kChunks = epi_chunks(kEpiWarps);
-  constexpr bool kEpiDoubleBuffer = kEpiWarps == 8;
-  extern __shared__ __align__(1024) unsigned char smem[];
-  __nv_bfloat16* sA = reinterpret_cast<__nv_bfloat16*>(smem);
-  __nv_bfloat16* sW = reinterpret_cast<__nv_bfloat16*>(smem + (size_t)STAGES * A_STAGE_BYTES);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)STAGES * (A_STAGE_BYTES + W_STAGE_BYTES));
-  uint64_t* full = bars;                 // [STAGES]
-  uint64_t* empty = bars + STAGES;       // [STAGES]
-  uint64_t* tfull = bars + 2 * STAGES;   // [2]
-  uint64_t* tempty = tfull + 2;          // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < STAGES; ++i) { sr_mbar_init(&full[i], 1); sr_mbar_init(&empty[i], 1); }
-    for (int i = 0; i < 2; ++i) { sr_mbar_init(&tfull[i], 1); sr_mbar_init(&tempty[i], kEpiWarps); }
-    sr_fence_barrier_init();
-  }
-  if (warp == 1) {  // TMEM: all 512 columns (two 256-column accumulators)
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                     sr_smem_u32(tmem_slot)),
-                 "r"(512)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  long long Mrows = a.M;
-  int MTe = a.MT;
-  if (a.m_dev != nullptr) {
-    const long long md = (long long)(*a.m_dev);
-    Mrows = md < a.M ? md : a.M;
-    MTe = (int)((Mrows + BM - 1) / BM);
-  }
-  const long long ntiles = (long long)MTe * a.NT;
-
-  if (warp == 0) {
-    // ------------------------------------------------------------------ TMA producer
-    if (lane == 0) {
-      int slot = 0;
-      uint32_t phase = 0;
-      for (long long t = blockIdx.x; t < ntiles; t += gridDim.x) {
-        const long long mt = t / a.NT;
-        const int nt = (int)(t % a.NT);
-        for (int kc = 0; kc < a.KC; ++kc) {
-          sr_mbar_wait(&empty[slot], phase ^ 1u);
-#ifdef SR_TC_DBG_NOLOAD   // tuning knock-out (tools/tc_diag.py): no operand traffic
-          sr_mbar_arrive(&full[slot]);
-#else
-          sr_mbar_arrive_expect_tx(&full[slot], A_STAGE_BYTES + W_STAGE_BYTES);
-          sr_bulk_g2s(sA + (size_t)slot * A_STAGE, a.A + a_tile_off(mt, kc, a.KC, 0), A_STAGE_BYTES, &full[slot]);
-          sr_bulk_g2s(sW + (size_t)slot * W_STAGE, a.W + w_tile_off(nt, kc, a.KC, 0), W_STAGE_BYTES, &full[slot]);
-#endif
-          if (++slot == STAGES) { slot = 0; phase ^= 1u; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer
-    if (lane == 0) {
-      int slot = 0;
-      uint32_t phase = 0;
-      int buf = 0;
-      uint32_t bphase = 0;
-      // plane pairs, smallest contributions first
-      constexpr int kTerms = kPlanes == 2 ? 3 : 6;
-      const int pa[6] = {0, 1, 0, 2, 1, 0};   // 2 planes: (a0,w1) (a1,w0) (a0,w0)
-      const int pw[6] = {1, 0, 0, 0, 1, 0};   // 3 planes: see below
-      const int pa3[6] = {0, 2, 1, 0, 1, 0};
-      const int pw3[6] = {2, 0, 1, 1, 0, 0};
-      for (long long t = blockIdx.x; t < ntiles; t += gridDim.x) {
-        const int nt = (int)(t % a.NT);
-        // N of this tile's MMAs: the GEMM's remaining columns rounded up to the instruction granule
-        int mma_n = a.n_gemm - nt * BN;
-        mma_n = mma_n >= BN ? BN : ((mma_n + 15) & ~15);
-        const uint32_t idesc = kIdescBase | ((uint32_t)(mma_n >> 3) << 17);
-        sr_mbar_wait(&tempty[buf], bphase ^ 1u);  // epilogue has drained this accumulator
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + (uint32_t)buf * BN;
-        uint32_t accumulate = 0;
-        for (int kc = 0; kc < a.KC; ++kc) {
-          sr_mbar_wait(&full[slot], phase);
-          tc_fence_after();
-          const uint32_t abase = sr_smem_u32(sA + (size_t)slot * A_STAGE);
-          const uint32_t wbase = sr_smem_u32(sW + (size_t)slot * W_STAGE);
-#ifdef SR_TC_DBG_NOMMA    // tuning knock-out: 1/16 of the MMAs
-          if (kc == 0)
-#endif
-#pragma unroll
-          for (int q = 0; q < kTerms; ++q) {
-#pragma unroll
-            for (int j = 0; j < BK / 16; ++j) {
-              // K = 16 per MMA = two 8-wide core matrices: advance two LBO steps per j
-              const int qa = kPlanes == 2 ? pa[q] : pa3[q], qw = kPlanes == 2 ? pw[q] : pw3[q];
-              const uint64_t ad = make_desc(abase + qa * (A_PLANE * 2) + j * 2 * (BM * 16), BM * 16, 128);
-              const uint64_t bd = make_desc(wbase + qw * (W_PLANE * 2) + j * 2 * (BN * 16), BN * 16, 128);
-              mma_bf16(tmem_d, ad, bd, idesc, accumulate);
-              accumulate = 1;
-            }
-          }
-          mma_commit(&empty[slot]);  // frees the smem stage when these MMAs have read it
-          if (++slot == STAGES) { slot = 0; phase ^= 1u; }
-        }
-        mma_commit(&tfull[buf]);     // accumulator complete
-        if (++buf == 2) { buf = 0; bphase ^= 1u; }
-      }
-    }
-  } else {
-    // ------------------------------------------------------------------ epilogue (warps 2..9)
-    const int q = warp & 3;                 // TMEM lane quarter this warp may access
-    const int half = (warp - 2) >> 2;       // which half of the 256 accumulator columns
-    EpiRow r;
-    r.row_in_tile = q * 32 + lane;
-    r.lane = lane;
-    r.is_val = (CH == 1) || ((lane & 3) == 0);
-    r.ds_ld = (size_t)a.NT * BN;
-    int buf = 0;
-    uint32_t bphase = 0;
-    for (long long t = blockIdx.x; t < ntiles; t += gridDim.x) {
-      r.mt = t / a.NT;
-      r.nt = (int)(t % a.NT);
-      r.row = r.mt * BM + r.row_in_tile;
-      r.row_ok = r.row < Mrows;
-      const int c_base = r.nt * BN + half * kPartCols;
-#ifdef SR_TC_DBG_NOEPI    // tuning knock-out: accumulators are drained without being read
-      const int n_live = 0;
-      if (t >= 0) r.row_ok = false;
-#else
-      const int n_live = (a.n_gemm - c_base + 31) >> 5;   // chunks of this warp's half that hold GEMM columns
-#endif
-      sr_mbar_wait(&tfull[buf], bphase);
-      tc_fence_after();
-      const uint32_t taddr0 = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)buf * BN + half * kPartCols;
-      if constexpr (CH == 1 && !MUL && kEpiDoubleBuffer) {
-        // two register buffers: the TMEM load of chunk i+1 is in flight while chunk i is processed
-        uint32_t va[32], vb[32];
-        if (n_live > 0) tmem_ld32_async(taddr0, va);
-#pragma unroll
-        for (int i = 0; i < kChunks; i += 2) {
-          if (i < n_live) tmem_wait(va);
-          if (i + 1 < n_live) tmem_ld32_async(taddr0 + (i + 1) * 32, vb);
-          epi_chunk<ACT, CH, MUL>(a, r, va, half * kChunks + i, i < n_live);
-          if (i + 1 < n_live) tmem_wait(vb);
-          if (i + 2 < kChunks && i + 2 < n_live) tmem_ld32_async(taddr0 + (i + 2) * 32, va);
-          epi_chunk<ACT, CH, MUL>(a, r, vb, half * kChunks + i + 1, i + 1 < n_live);
-        }
-      } else {
-        for (int i = 0; i < kChunks; ++i) {
-          uint32_t v[32];
-          // the chunk's global operands are requested inside epi_chunk BEFORE it waits for the TMEM load
-          if (i < n_live) tmem_ld32_async(taddr0 + i * 32, v);
-          epi_chunk<ACT, CH, MUL, kEpiWarps == 8>(a, r, v, half * kChunks + i, i < n_live, i < n_live);
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) sr_mbar_arrive(&tempty[buf]);
-      if (++buf == 2) { buf = 0; bphase ^= 1u; }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
-  }
-}
-
-
-// ---- CTA-pair variant (cta_group::2) ----------------------------------------------------------
-// Two CTAs of a cluster (the two SMs of a TPC) share one 256 x 256 output tile: CTA r owns rows
-// [128 r, 128 r + 128) (its own A tile and TMEM accumulator) and stages only HALF of the weight tile
-// (columns [128 r, +128)); the leader (rank 0) issues `tcgen05.mma.cta_group::2` with M = 256, which reads
-// A from each CTA's own shared memory and the two B halves from both.  Per SM that is 4 + 4 KB of operand
-// reads per MMA instead of 4 + 8 and 32 KB instead of 48 KB of TMA fill per stage -- the single-CTA
-// kernel is bound by exactly that shared-memory traffic (profiles/r01b_summary.md).
-//   barriers (each CTA's own shared memory unless noted):
-//     full[s]   own TMA bytes of stage s landed                    (producer expect_tx, count 1)
-//     pfull[s]  LEADER only: the peer's stage s landed             (remote arrive by the peer's relay thread)
-//     empty[s]  stage s consumed: leader's tcgen05.commit multicast to both CTAs
-//     tfull[b]  accumulator b complete: leader's commit multicast to both CTAs
-//     tempty[b] LEADER only: accumulator b drained by the epilogue warps of BOTH CTAs (2 x kEpiWarps)
-constexpr int P_STAGES = 6;
-constexpr int PB_PLANE = 128 * BK;                        // half weight tile plane: 128 rows x 32 k
-constexpr int PB_STAGE = kPlanes * PB_PLANE;              // 16 KB (2 planes)
-constexpr uint32_t PB_STAGE_BYTES = PB_STAGE * 2;
-constexpr size_t kSmemPair = (size_t)P_STAGES * (A_STAGE_BYTES + PB_STAGE_BYTES) + 512;
-constexpr uint32_t kIdescPair = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(256 >> 4) << 24);
-
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// arrive on the barrier at the same offset in CTA `rank` of the cluster
-__device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t rank) {
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}" ::"r"(sr_smem_u32(bar)),
-      "r"(rank)
-      : "memory");
-}
-// wait on a local barrier that remote CTAs (or the async proxy of the pair) arrive on.  Default (CTA-scope)
-// semantics on purpose: nothing written through the generic proxy by the partner is read here (operands
-// arrive by TMA, accumulators through TMEM + tcgen05 fences), and a cluster-scope acquire compiles to
-// MEMBAR.ALL.GPU + CCTL.IVALL in every poll -- measured 0.43 ms instead of 0.33 ms per layer.
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "WAIT_LOOP_C:\n"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-      "@p bra.uni WAIT_DONE_C;\n"
-      "bra.uni WAIT_LOOP_C;\n"
-      "WAIT_DONE_C:\n"
-      "}\n" ::"r"(sr_smem_u32(bar)),
-      "r"(parity)
-      : "memory");
-}
-__device__ __forceinline__ void mma_bf16_pair(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                              uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void mma_commit_pair(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          sr_smem_u32(bar)),
-      "h"((uint16_t)3)
-      : "memory");
-}
-
-template <int ACT, int CH, bool MUL>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(epi_threads(MUL), 1)
-    tc_layer_pair_kernel(const __grid_constant__ LayerArgs a) {
-  constexpr int kEpiWarps = epi_warps(MUL), kPartCols = epi_part_cols(kEpiWarps), kChunks = epi_chunks(kEpiWarps);
-  constexpr bool kEpiDoubleBuffer = kEpiWarps == 8;
-  extern __shared__ __align__(1024) unsigned char smem[];
-  __nv_bfloat16* sA = reinterpret_cast<__nv_bfloat16*>(smem);
-  __nv_bfloat16* sW = reinterpret_cast<__nv_bfloat16*>(smem + (size_t)P_STAGES * A_STAGE_BYTES);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)P_STAGES * (A_STAGE_BYTES + PB_STAGE_BYTES));
-  uint64_t* full = bars;                    // [P_STAGES]
-  uint64_t* pfull = bars + P_STAGES;        // [P_STAGES]  (used in the leader)
-  uint64_t* empty = bars + 2 * P_STAGES;    // [P_STAGES]
-  uint64_t* tfull = bars + 3 * P_STAGES;    // [2]
-  uint64_t* tempty = tfull + 2;             // [2]         (used in the leader)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < P_STAGES; ++i) { sr_mbar_init(&full[i], 1); sr_mbar_init(&pfull[i], 1); sr_mbar_init(&empty[i], 1); }
-    for (int i = 0; i < 2; ++i) { sr_mbar_init(&tfull[i], 1); sr_mbar_init(&tempty[i], 2 * kEpiWarps); }
-    sr_fence_barrier_init();
-  }
-  if (warp == 1) {  // TMEM: all 512 columns in both CTAs (same warp id in both, cta_group::2)
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                     sr_smem_u32(tmem_slot)),
-                 "r"(512)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  cluster_sync_all();      // barrier inits of both CTAs visible before any remote arrive / multicast commit
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  long long Mrows = a.M;
-  int MTe = a.MT;
-  if (a.m_dev != nullptr) {
-    const long long md = (long long)(*a.m_dev);
-    Mrows = md < a.M ? md : a.M;
-    MTe = (int)((Mrows + BM - 1) / BM);
-  }
-  const long long npt = (long long)((MTe + 1) / 2) * a.NT;     // pair tiles (256 rows x 256 columns)
-  const long long pair_id = blockIdx.x >> 1, npairs = gridDim.x >> 1;
-
-  if (warp == 0) {
-    // ------------------------------------------------------------------ TMA producer (both CTAs)
-    if (lane == 0) {
-      int slot = 0;
-      uint32_t phase = 0;
-      for (long long t = pair_id; t < npt; t += npairs) {
-        const long long mt = (t / a.NT) * 2 + rank;
-        const int nt = (int)(t % a.NT);
-        const bool have_a = mt < MTe;       // odd tile count: the peer's rows of the last pair do not exist
-        for (int kc = 0; kc < a.KC; ++kc) {
-          mbar_wait_cluster(&empty[slot], phase ^ 1u);
-#ifdef SR_TC_DBG_NOLOAD
-          sr_mbar_arrive(&full[slot]);
-#else
-          sr_mbar_arrive_expect_tx(&full[slot], (have_a ? A_STAGE_BYTES : 0u) + PB_STAGE_BYTES);
-          if (have_a)
-            sr_bulk_g2s(sA + (size_t)slot * A_STAGE, a.A + a_tile_off(mt, kc, a.KC, 0), A_STAGE_BYTES, &full[slot]);
-          // this CTA's half of the weight tile (columns [128 rank, +128)): one contiguous block of the pair layout
-          sr_bulk_g2s(sW + (size_t)slot * PB_STAGE,
-                      a.Wp + (((size_t)nt * a.KC + kc) * 2 + rank) * PB_STAGE, PB_STAGE_BYTES, &full[slot]);
-#endif
-          if (++slot == P_STAGES) { slot = 0; phase ^= 1u; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      int slot = 0;
-      uint32_t phase = 0;
-      if (!leader) {
-        // -------------------------------------------------------------- peer: relay "my stage landed"
-        for (long long t = pair_id; t < npt; t += npairs) {
-          for (int kc = 0; kc < a.KC; ++kc) {
-            sr_mbar_wait(&full[slot], phase);
-            mbar_arrive_remote(&pfull[slot], 0);
-            if (++slot == P_STAGES) { slot = 0; phase ^= 1u; }
-          }
-        }
-      } else {
-        // -------------------------------------------------------------- leader: MMA issuer for the pair
-        int buf = 0;
-        uint32_t bphase = 0;
-        constexpr int kTerms = kPlanes == 2 ? 3 : 6;
-        const int pa[6] = {0, 1, 0, 2, 1, 0};
-        const int pw[6] = {1, 0, 0, 0, 1, 0};
-        const int pa3[6] = {0, 2, 1, 0, 1, 0};
-        const int pw3[6] = {2, 0, 1, 1, 0, 0};
-        for (long long t = pair_id; t < npt; t += npairs) {
-          const int nt = (int)(t % a.NT);
-          (void)nt;
-          const uint32_t idesc = kIdescPair | ((uint32_t)(BN >> 3) << 17);
-          mbar_wait_cluster(&tempty[buf], bphase ^ 1u);
-          tc_fence_after();
-          const uint32_t tmem_d = tmem_base + (uint32_t)buf * BN;
-          uint32_t accumulate = 0;
-          for (int kc = 0; kc < a.KC; ++kc) {
-            sr_mbar_wait(&full[slot], phase);
-#ifndef SR_TC_DBG_NOPFULL   // tuning knock-out: do not wait for the peer's stage
-            mbar_wait_cluster(&pfull[slot], phase);
-#endif
-            tc_fence_after();
-            const uint32_t abase = sr_smem_u32(sA + (size_t)slot * A_STAGE);
-            const uint32_t wbase = sr_smem_u32(sW + (size_t)slot * PB_STAGE);
-#ifdef SR_TC_DBG_NOMMA
-            if (kc == 0)
-#endif
-#pragma unroll
-            for (int q = 0; q < kTerms; ++q) {
-#pragma unroll
-              for (int j = 0; j < BK / 16; ++j) {
-                const int qa = kPlanes == 2 ? pa[q] : pa3[q], qw = kPlanes == 2 ? pw[q] : pw3[q];
-                const uint64_t ad = make_desc(abase + qa * (A_PLANE * 2) + j * 2 * (BM * 16), BM * 16, 128);
-                const uint64_t bd = make_desc(wbase + qw * (PB_PLANE * 2) + j * 2 * (128 * 16), 128 * 16, 128);
-                mma_bf16_pair(tmem_d, ad, bd, idesc, accumulate);
-                accumulate = 1;
-              }
-            }
-            mma_commit_pair(&empty[slot]);
-            if (++slot == P_STAGES) { slot = 0; phase ^= 1u; }
-          }
-          mma_commit_pair(&tfull[buf]);
-          if (++buf == 2) { buf = 0; bphase ^= 1u; }
-        }
-      }
-    }
-  } else {
-    // ------------------------------------------------------------------ epilogue (warps 2..9, both CTAs)
-    const int q = warp & 3;
-    const int half = (warp - 2) >> 2;
-    EpiRow r;
-    r.row_in_tile = q * 32 + lane;
-    r.lane = lane;
-    r.is_val = (CH == 1) || ((lane & 3) == 0);
-    r.ds_ld = (size_t)a.NT * BN;
-    int buf = 0;
-    uint32_t bphase = 0;
-    for (long long t = pair_id; t < npt; t += npairs) {
-      r.mt = (t / a.NT) * 2 + rank;
-      r.nt = (int)(t % a.NT);
-      r.row = r.mt * BM + r.row_in_tile;
-      r.row_ok = r.row < Mrows;
-#ifdef SR_TC_DBG_NOEPI
-      const bool have_rows = false;
-#else
-      const bool have_rows = r.mt < MTe;
-#endif
-      const int c_base = r.nt * BN + half * kPartCols;
-      const int n_live = have_rows ? (a.n_gemm - c_base + 31) >> 5 : 0;
-      mbar_wait_cluster(&tfull[buf], bphase);
-      tc_fence_after();
-      const uint32_t taddr0 = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)buf * BN + half * kPartCols;
-      if (!have_rows) {
-        // phantom row tile of an odd tile count: nothing to read or write
-      } else if constexpr (CH == 1 && !MUL && kEpiDoubleBuffer) {
-        uint32_t va[32], vb[32];
-        if (n_live > 0) tmem_ld32_async(taddr0, va);
-#pragma unroll
-        for (int i = 0; i < kChunks; i += 2) {
-          if (i < n_live) tmem_wait(va);
-          if (i + 1 < n_live) tmem_ld32_async(taddr0 + (i + 1) * 32, vb);
-          epi_chunk<ACT, CH, MUL>(a, r, va, half * kChunks + i, i < n_live);
-          if (i + 1 < n_live) tmem_wait(vb);
-          if (i + 2 < kChunks && i + 2 < n_live) tmem_ld32_async(taddr0 + (i + 2) * 32, va);
-          epi_chunk<ACT, CH, MUL>(a, r, vb, half * kChunks + i + 1, i + 1 < n_live);
-        }
-      } else {
-        for (int i = 0; i < kChunks; ++i) {
-          uint32_t v[32];
-          // the chunk's global operands are requested inside epi_chunk BEFORE it waits for the TMEM load
-          if (i < n_live) tmem_ld32_async(taddr0 + i * 32, v);
-          epi_chunk<ACT, CH, MUL, kEpiWarps == 8>(a, r, v, half * kChunks + i, i < n_live, i < n_live);
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_remote(&tempty[buf], 0);   // the leader's barrier counts both CTAs' warps
-      if (++buf == 2) { buf = 0; bphase ^= 1u; }
-    }
-  }
-  tc_fence_before();
-  cluster_sync_all();      // no CTA leaves (or frees TMEM) while its partner may still touch it
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
-  }
-}
-
-// ---- whole-sweep kernel: all layers of a forward or reverse sweep in ONE launch ---------------------------
-// A CTA pair keeps its row tiles through every layer of the sweep: pair p owns the row-pair tiles
-// {p, p + npairs, ...} (256 rows each) in EVERY step.  The activations a step's epilogue writes for rows R are
-// exactly what the same CTA loads as the next step's A operand for rows R, so the only dependency between steps
-// is inside a CTA: the producer waits until the eight epilogue warps have finished the previous step on that row
-// tile (per-warp progress counters in shared memory, release / acquire, with a generic->async proxy fence on both
-// sides because the tiles are written with st.global and read back by the bulk-copy engine).  No grid or cluster
-// barrier between layers, one TMEM allocation, one barrier set-up and one launch ramp per SWEEP instead of per
-// layer; the smem ring and the two TMEM accumulators simply keep rolling across the layer boundary, so the first
-// MMAs of step l+1 overlap the last epilogue of step l whenever a pair owns more than one row tile.
+// ---- the layer kernel: all layers of a forward or reverse sweep in ONE launch ----------------------------------
+// A CTA keeps its row tiles through every layer of the sweep: CTA c owns the row tiles {c, c + grid, ...} in EVERY
+// step.  The activations a step's epilogue writes for rows R are exactly what the same CTA loads as the next step's A
+// operand for rows R, so the only dependency between steps is inside a CTA: the producer waits until the eight
+// epilogue warps have finished the previous step on that row tile (per-warp progress counters in shared memory,
+// release / acquire, with a generic->async proxy fence on both sides because the tiles are written with st.global and
+// read back by the bulk-copy engine).  No grid barrier between layers, one barrier set-up and one launch ramp per
+// SWEEP instead of per layer; the smem ring keeps rolling across the layer boundary, so the loads of step l+1 overlap
+// the last epilogue of step l.  A single layer (sr_tc_linear) is a sweep of one step.
 // Narrow steps (N < 256: the SDF's last layer, the input gradient of the reverse sweep) run as one N = 256 tile on
 // zero-padded weight rows.  Buffers that hold tiles of different widths must be distinct: tile (mt, kc) sits at
 // (mt * KC + kc), so two layouts of one buffer alias ACROSS row tiles (the host wrapper checks this).
+//
+// Roles (3 warpgroups): warpgroup 0 = TMA producer (one thread), warpgroups 1 and 2 = rows [0, 64) and [64, 128) of
+// the 128 x 256 output tile: wgmma m64n256k16 with fp32 accumulators in registers (128 per thread), then the
+// epilogue of the same rows.  The accumulator goes through shared memory (128 columns at a time) so that each
+// epilogue thread owns one row and 32 consecutive columns per chunk: the four rows of a point (value + 3 tangents)
+// sit in four consecutive lanes.
 constexpr int kMaxSteps = 12;
-static_assert(kPlanes == 2, "the whole-sweep kernel issues the 3-term (2-plane) product");
+constexpr int kConsumerWGs = 2;
+constexpr int kThreads = 128 * (1 + kConsumerWGs);
+constexpr int kEpiWarps = 4 * kConsumerWGs;
+constexpr int STG_LD = 132;                 // staging row pitch (floats): conflict-free float4 row reads
+constexpr int STG_FLOATS = 64 * STG_LD;     // per consumer warpgroup: 64 rows x 128 columns
+constexpr size_t kSmem = (size_t)STAGES * (A_STAGE_BYTES + W_STAGE_BYTES) + (size_t)kConsumerWGs * STG_FLOATS * 4 + 256;
+static_assert(kSmem <= 227 * 1024, "shared memory of one H100 block");
 struct StepArgs {
   LayerArgs la;
   int act;       // SR_ACT_* of a forward step / of the PREVIOUS layer for a reverse (mul) step
@@ -796,69 +365,47 @@ __device__ __forceinline__ uint32_t ld_acquire_smem(const uint32_t* p) {
   return v;
 }
 
-// one accumulator (this warp's 32 lanes x its 128-column half) -> epilogue
-template <int ACT, int CH, bool MUL, int EW, bool DB = true>
-__device__ __forceinline__ void epi_item(const LayerArgs& a, const EpiRow& r, uint32_t taddr0, int n_live, int half) {
-  constexpr int kChunks = epi_chunks(EW);
-  if constexpr (CH == 1 && !MUL && DB && EW == 8) {
-    uint32_t va[32], vb[32];
-    if (n_live > 0) tmem_ld32_async(taddr0, va);
+// One k chunk of this warpgroup's 64 x 256 tile: the split-bf16 product terms, plane pairs smallest contributions
+// first -- 2 planes: (a0,w1) (a1,w0) (a0,w0); 3 planes: (a0,w2) (a2,w0) (a1,w1) (a0,w1) (a1,w0) (a0,w0).
+// abase = this warpgroup's first row group of the A stage, wbase = the W stage.
+template <bool FIRST>
+__device__ __forceinline__ void mma_chunk(float (&acc)[128], uint32_t abase, uint32_t wbase) {
+  constexpr int kTerms = kPlanes == 2 ? 3 : 6;
+  const int pa[6] = {0, 1, 0, 2, 1, 0}, pw[6] = {1, 0, 0, 0, 1, 0};
+  const int pa3[6] = {0, 2, 1, 0, 1, 0}, pw3[6] = {2, 0, 1, 1, 0, 0};
 #pragma unroll
-    for (int i = 0; i < kChunks; i += 2) {
-      if (i < n_live) tmem_wait(va);
-      if (i + 1 < n_live) tmem_ld32_async(taddr0 + (i + 1) * 32, vb);
-      epi_chunk<ACT, CH, MUL>(a, r, va, half * kChunks + i, i < n_live);
-      if (i + 1 < n_live) tmem_wait(vb);
-      if (i + 2 < kChunks && i + 2 < n_live) tmem_ld32_async(taddr0 + (i + 2) * 32, va);
-      epi_chunk<ACT, CH, MUL>(a, r, vb, half * kChunks + i + 1, i + 1 < n_live);
-    }
-  } else {
-    for (int i = 0; i < kChunks; ++i) {
-      uint32_t v[32];
-      if (i < n_live) tmem_ld32_async(taddr0 + i * 32, v);
-      epi_chunk<ACT, CH, MUL, EW == 8>(a, r, v, half * kChunks + i, i < n_live, i < n_live);
+  for (int q = 0; q < kTerms; ++q) {
+#pragma unroll
+    for (int jj = 0; jj < BK / 16; ++jj) {
+      // K = 16 per MMA = two 8-wide core matrices: advance two LBO steps per jj
+      const int qa = kPlanes == 2 ? pa[q] : pa3[q], qw = kPlanes == 2 ? pw[q] : pw3[q];
+      const uint64_t ad = make_desc(abase + qa * (A_PLANE * 2) + jj * 2 * (BM * 16), BM * 16, 128);
+      const uint64_t bd = make_desc(wbase + qw * (W_PLANE * 2) + jj * 2 * (BN * 16), BN * 16, 128);
+      if (FIRST && q == 0 && jj == 0) wgmma_m64n256k16<0, 0, true>(acc, ad, bd);
+      else wgmma_m64n256k16<0, 0, false>(acc, ad, bd);
     }
   }
 }
 
 // <ACT, MUL>: activation / mode of every step but (optionally) the last -- the two epilogues a sweep needs
 template <int ACT, int CH, bool MUL>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(epi_threads(MUL), 1)
-    tc_sweep_pair_kernel(const __grid_constant__ SweepArgs sw) {
-  constexpr int kEpiWarps = epi_warps(MUL), kPartCols = epi_part_cols(kEpiWarps);
+__global__ void __launch_bounds__(kThreads, 1) tc_sweep_kernel(const __grid_constant__ SweepArgs sw) {
   extern __shared__ __align__(1024) unsigned char smem[];
   __nv_bfloat16* sA = reinterpret_cast<__nv_bfloat16*>(smem);
-  __nv_bfloat16* sW = reinterpret_cast<__nv_bfloat16*>(smem + (size_t)P_STAGES * A_STAGE_BYTES);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)P_STAGES * (A_STAGE_BYTES + PB_STAGE_BYTES));
-  uint64_t* full = bars;                    // [P_STAGES]
-  uint64_t* pfull = bars + P_STAGES;        // [P_STAGES]  (used in the leader)
-  uint64_t* empty = bars + 2 * P_STAGES;    // [P_STAGES]
-  uint64_t* tfull = bars + 3 * P_STAGES;    // [2]
-  uint64_t* tempty = tfull + 2;             // [2]         (used in the leader)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
-  uint32_t* done = tmem_slot + 2;           // [kEpiWarps] items finished by each epilogue warp of THIS CTA
+  __nv_bfloat16* sW = reinterpret_cast<__nv_bfloat16*>(smem + (size_t)STAGES * A_STAGE_BYTES);
+  float* stg = reinterpret_cast<float*>(smem + (size_t)STAGES * (A_STAGE_BYTES + W_STAGE_BYTES));
+  uint64_t* bars = reinterpret_cast<uint64_t*>(stg + kConsumerWGs * STG_FLOATS);
+  uint64_t* full = bars;                    // [STAGES] operands of the stage landed (producer expect_tx)
+  uint64_t* empty = bars + STAGES;          // [STAGES] the MMAs of every consumer warp have read the stage
+  uint32_t* done = reinterpret_cast<uint32_t*>(empty + STAGES);   // [kEpiWarps] items finished by each epilogue warp
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7;
   if (threadIdx.x == 0) {
-    for (int i = 0; i < P_STAGES; ++i) { sr_mbar_init(&full[i], 1); sr_mbar_init(&pfull[i], 1); sr_mbar_init(&empty[i], 1); }
-    for (int i = 0; i < 2; ++i) { sr_mbar_init(&tfull[i], 1); sr_mbar_init(&tempty[i], 2 * kEpiWarps); }
+    for (int i = 0; i < STAGES; ++i) { sr_mbar_init(&full[i], 1); sr_mbar_init(&empty[i], kEpiWarps); }
     for (int i = 0; i < kEpiWarps; ++i) done[i] = 0u;
     sr_fence_barrier_init();
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                     sr_smem_u32(tmem_slot)),
-                 "r"(512)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();         // `done` zeroed before any role reads it
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  __syncthreads();
   const LayerArgs& a0 = sw.step[0].la;
   long long Mrows = a0.M;
   int MTe = a0.MT;
@@ -867,14 +414,16 @@ __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(epi_threads(MUL), 1)
     Mrows = md < a0.M ? md : a0.M;
     MTe = (int)((Mrows + BM - 1) / BM);
   }
-  const int nrp = (MTe + 1) / 2;                                   // row-pair tiles (256 rows)
-  const int pair_id = blockIdx.x >> 1, npairs = gridDim.x >> 1;
-  const int J = pair_id < nrp ? (nrp - pair_id + npairs - 1) / npairs : 0;   // row-pair tiles of this pair
+  const int cta = blockIdx.x, ncta = gridDim.x;
+  const int J = cta < MTe ? (MTe - cta + ncta - 1) / ncta : 0;   // row tiles of this CTA
   const int L = sw.L;
 
-  if (warp == 0) {
-    // ------------------------------------------------------------------ TMA producer (both CTAs)
-    if (lane == 0) {
+  // 384 threads at one block per SM start with 168 registers each; the producer warpgroup hands most of its share to
+  // the consumers (128 accumulators + epilogue state per thread): 128 x 40 + 256 x 232 <= 65 536
+  if (wg == 0) {
+    // ------------------------------------------------------------------ TMA producer
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (threadIdx.x == 0) {
       int slot = 0;
       uint32_t phase = 0;
       uint32_t items_before = 0;            // items of the steps before the previous one
@@ -882,136 +431,112 @@ __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(epi_threads(MUL), 1)
         const LayerArgs& a = sw.step[l].la;
         const int NTp = l > 0 ? sw.step[l - 1].la.NT : 0;
         for (int j = 0; j < J; ++j) {
-          const long long mt = (long long)(pair_id + j * npairs) * 2 + rank;
-          const bool have_a = mt < MTe;
+          const long long mt = (long long)cta + (long long)j * ncta;
           for (int nt = 0; nt < a.NT; ++nt) {
             for (int kc = 0; kc < a.KC; ++kc) {
-              mbar_wait_cluster(&empty[slot], phase ^ 1u);
-              sr_mbar_arrive_expect_tx(&full[slot], (have_a ? A_STAGE_BYTES : 0u) + PB_STAGE_BYTES);
-              sr_bulk_g2s(sW + (size_t)slot * PB_STAGE,
-                          a.Wp + (((size_t)nt * a.KC + kc) * 2 + rank) * PB_STAGE, PB_STAGE_BYTES, &full[slot]);
+              sr_mbar_wait(&empty[slot], phase ^ 1u);
+              sr_mbar_arrive_expect_tx(&full[slot], A_STAGE_BYTES + W_STAGE_BYTES);
+              sr_bulk_g2s(sW + (size_t)slot * W_STAGE, a.W + w_tile_off(nt, kc, a.KC, 0), W_STAGE_BYTES, &full[slot]);
               if (l > 0 && nt == 0 && kc == 0) {
-                // rows of tile j: every n-tile of the previous step must have left the epilogue (this CTA's warps)
+                // rows of tile j: every n-tile of the previous step must have left the epilogue
                 const uint32_t need = items_before + (uint32_t)(j + 1) * (uint32_t)NTp;
                 for (int w = 0; w < kEpiWarps; ++w)
                   while (ld_acquire_smem(&done[w]) < need) {}
                 fence_proxy_async();
               }
-              if (have_a)
-                sr_bulk_g2s(sA + (size_t)slot * A_STAGE, a.A + a_tile_off(mt, kc, a.KC, 0), A_STAGE_BYTES, &full[slot]);
-              if (++slot == P_STAGES) { slot = 0; phase ^= 1u; }
+              sr_bulk_g2s(sA + (size_t)slot * A_STAGE, a.A + a_tile_off(mt, kc, a.KC, 0), A_STAGE_BYTES, &full[slot]);
+              if (++slot == STAGES) { slot = 0; phase ^= 1u; }
             }
           }
         }
         if (l > 0) items_before += (uint32_t)J * (uint32_t)NTp;
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      int slot = 0;
-      uint32_t phase = 0;
-      if (!leader) {
-        for (int l = 0; l < L; ++l) {
-          const LayerArgs& a = sw.step[l].la;
-          const int n_it = J * a.NT * a.KC;
-          for (int it = 0; it < n_it; ++it) {
-            sr_mbar_wait(&full[slot], phase);
-            mbar_arrive_remote(&pfull[slot], 0);
-            if (++slot == P_STAGES) { slot = 0; phase ^= 1u; }
-          }
-        }
-      } else {
-        int buf = 0;
-        uint32_t bphase = 0;
-        const int pa[3] = {0, 1, 0};
-        const int pw[3] = {1, 0, 0};
-        const uint32_t idesc = kIdescPair | ((uint32_t)(BN >> 3) << 17);
-        for (int l = 0; l < L; ++l) {
-          const LayerArgs& a = sw.step[l].la;
-          const int n_items = J * a.NT;
-          for (int item = 0; item < n_items; ++item) {
-            mbar_wait_cluster(&tempty[buf], bphase ^ 1u);
-            tc_fence_after();
-            const uint32_t tmem_d = tmem_base + (uint32_t)buf * BN;
-            uint32_t accumulate = 0;
-            for (int kc = 0; kc < a.KC; ++kc) {
-              sr_mbar_wait(&full[slot], phase);
-              mbar_wait_cluster(&pfull[slot], phase);
-              tc_fence_after();
-              const uint32_t abase = sr_smem_u32(sA + (size_t)slot * A_STAGE);
-              const uint32_t wbase = sr_smem_u32(sW + (size_t)slot * PB_STAGE);
-#pragma unroll
-              for (int q = 0; q < 3; ++q) {
-#pragma unroll
-                for (int jj = 0; jj < BK / 16; ++jj) {
-                  const uint64_t ad = make_desc(abase + pa[q] * (A_PLANE * 2) + jj * 2 * (BM * 16), BM * 16, 128);
-                  const uint64_t bd = make_desc(wbase + pw[q] * (PB_PLANE * 2) + jj * 2 * (128 * 16), 128 * 16, 128);
-                  mma_bf16_pair(tmem_d, ad, bd, idesc, accumulate);
-                  accumulate = 1;
-                }
-              }
-              mma_commit_pair(&empty[slot]);
-              if (++slot == P_STAGES) { slot = 0; phase ^= 1u; }
-            }
-            mma_commit_pair(&tfull[buf]);
-            if (++buf == 2) { buf = 0; bphase ^= 1u; }
-          }
-        }
-      }
-    }
   } else {
-    // ------------------------------------------------------------------ epilogue (warps 2..9, both CTAs)
-    const int q = warp & 3;
-    const int half = (warp - 2) >> 2;
+    // ------------------------------------------------------------------ MMA + epilogue (warpgroups 1, 2)
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    const int cw = wg - 1;                  // rows [64 cw, 64 cw + 64) of the row tile
+    const int wq = warp & 3;                // warp in the warpgroup
+    const int ew = 4 * cw + wq;             // epilogue warp index
+    float* st = stg + cw * STG_FLOATS;
+    float acc[128];
     EpiRow r;
-    r.row_in_tile = q * 32 + lane;
+    r.row_in_tile = cw * 64 + (wq & 1) * 32 + lane;
     r.lane = lane;
     r.is_val = (CH == 1) || ((lane & 3) == 0);
-    int buf = 0;
-    uint32_t bphase = 0;
+    int slot = 0;
+    uint32_t phase = 0;
     uint32_t items = 0;
     for (int l = 0; l < L; ++l) {
       const LayerArgs& a = sw.step[l].la;
       const bool plain = sw.last_plain && l == L - 1;
       r.ds_ld = (size_t)a.NT * BN;
       for (int j = 0; j < J; ++j) {
-        r.mt = (long long)(pair_id + j * npairs) * 2 + rank;
+        r.mt = (long long)cta + (long long)j * ncta;
         r.row = r.mt * BM + r.row_in_tile;
         r.row_ok = r.row < Mrows;
-        const bool have_rows = r.mt < MTe;
         for (int nt = 0; nt < a.NT; ++nt) {
           r.nt = nt;
-          const int c_base = nt * BN + half * kPartCols;
-          const int n_live = have_rows ? (a.n_gemm - c_base + 31) >> 5 : 0;
-          mbar_wait_cluster(&tfull[buf], bphase);
-          tc_fence_after();
-          const uint32_t taddr0 = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)buf * BN + half * kPartCols;
-          if (have_rows) {
-            if (plain) epi_item<SR_ACT_NONE, CH, false, kEpiWarps, false>(a, r, taddr0, n_live, half);
-            else epi_item<ACT, CH, MUL, kEpiWarps>(a, r, taddr0, n_live, half);
+          // the first k chunk overwrites the accumulator (it is dead from here back to the previous epilogue)
+          sr_mbar_wait(&full[slot], phase);
+          wgmma_fence();
+          mma_chunk<true>(acc, sr_smem_u32(sA + (size_t)slot * A_STAGE) + cw * 8 * 128,
+                          sr_smem_u32(sW + (size_t)slot * W_STAGE));
+          wgmma_commit();
+          int prev = slot;
+          if (++slot == STAGES) { slot = 0; phase ^= 1u; }
+          for (int kc = 1; kc < a.KC; ++kc) {
+            sr_mbar_wait(&full[slot], phase);
+            wgmma_fence();
+            mma_chunk<false>(acc, sr_smem_u32(sA + (size_t)slot * A_STAGE) + cw * 8 * 128,
+                             sr_smem_u32(sW + (size_t)slot * W_STAGE));
+            wgmma_commit();
+            wgmma_wait<1>();   // the previous stage's MMAs are complete: release it
+            if (lane == 0) sr_mbar_arrive(&empty[prev]);
+            prev = slot;
+            if (++slot == STAGES) { slot = 0; phase ^= 1u; }
           }
-          tc_fence_before();
+          wgmma_wait<0>();
+          if (lane == 0) sr_mbar_arrive(&empty[prev]);
+          // epilogue: 128 accumulator columns per pass through the staging buffer; warp wq handles rows
+          // 32 (wq & 1) + lane and the 64 columns 64 (wq >> 1) of each pass (two 32-column chunks)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int fr = 16 * wq + (lane >> 2), fc = 2 * (lane & 3);
+#pragma unroll
+            for (int i = 0; i < 16; ++i) {
+              *reinterpret_cast<float2*>(st + fr * STG_LD + 8 * i + fc) =
+                  make_float2(acc[4 * (16 * h + i)], acc[4 * (16 * h + i) + 1]);
+              *reinterpret_cast<float2*>(st + (fr + 8) * STG_LD + 8 * i + fc) =
+                  make_float2(acc[4 * (16 * h + i) + 2], acc[4 * (16 * h + i) + 3]);
+            }
+            warpgroup_sync(1 + cw);
+            const float* srow = st + ((wq & 1) * 32 + lane) * STG_LD + (wq >> 1) * 64;
+            for (int i = 0; i < 2; ++i) {
+              const int chunk = 4 * h + 2 * (wq >> 1) + i;
+              uint32_t v[32];
+#pragma unroll
+              for (int j4 = 0; j4 < 8; ++j4) {
+                const float4 t = reinterpret_cast<const float4*>(srow + 32 * i)[j4];
+                v[4 * j4] = __float_as_uint(t.x); v[4 * j4 + 1] = __float_as_uint(t.y);
+                v[4 * j4 + 2] = __float_as_uint(t.z); v[4 * j4 + 3] = __float_as_uint(t.w);
+              }
+              const bool live = nt * BN + chunk * 32 < a.n_gemm;
+              if (plain) epi_chunk<SR_ACT_NONE, CH, false>(a, r, v, chunk, live);
+              else epi_chunk<ACT, CH, MUL>(a, r, v, chunk, live);
+            }
+            warpgroup_sync(1 + cw);
+          }
           // this lane's tile stores -> visible to the bulk copies of the next step (nothing reads the last step's)
-          // (one fence + one progress update per ROW TILE: the next step needs all n-tiles of the row tile anyway;
-          //  fence.proxy.async is MEMBAR.GPU + FENCE.VIEW.ASYNC, i.e. it waits for this lane's stores)
+          // (one fence + one progress update per ROW TILE: the next step needs all n-tiles of the row tile anyway)
           ++items;
           const bool publish = nt == a.NT - 1 && l + 1 < L;
           if (publish && !(sw.dbg & 1)) fence_proxy_async();
           __syncwarp();
-          if (lane == 0) {
-            mbar_arrive_remote(&tempty[buf], 0);
-            if (publish) st_release_smem(&done[warp - 2], items);
-          }
-          if (++buf == 2) { buf = 0; bphase ^= 1u; }
+          if (publish && lane == 0) st_release_smem(&done[ew], items);
         }
       }
     }
-  }
-  tc_fence_before();
-  cluster_sync_all();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
   }
 }
 
@@ -1049,7 +574,7 @@ __global__ void pack_rows_kernel(const float* __restrict__ src, long long M, int
   }
 }
 
-// effective weights, fp32 row-major [N][K] (ld) -> tiled split-bf16 [NT][KC][planes][256x32] followed by the CTA-pair layout
+// effective weights, fp32 row-major [N][K] (ld) -> tiled split-bf16 [NT][KC][planes][256x32]
 __global__ void pack_weights_kernel(const float* __restrict__ w, int N, int K, int ld,
                                     __nv_bfloat16* __restrict__ dst, int NT, int KC) {
   const long long total = (long long)NT * BN * KC * 4;
@@ -1071,12 +596,6 @@ __global__ void pack_weights_kernel(const float* __restrict__ w, int N, int K, i
     const size_t off = (size_t)k8 * (BN * 8) + (size_t)(r >> 3) * 64 + (r & 7) * 8;
     *reinterpret_cast<uint4*>(dst + w_tile_off(nt, kc, KC, 0) + off) = *reinterpret_cast<uint4*>(p1);
     *reinterpret_cast<uint4*>(dst + w_tile_off(nt, kc, KC, 1) + off) = *reinterpret_cast<uint4*>(p2);
-    // second copy in the CTA-pair layout: [nt][kc][half][plane][k8][128 rows][8]
-    __nv_bfloat16* dp = dst + (size_t)NT * KC * W_STAGE + (((size_t)nt * KC + kc) * 2 + (r >> 7)) * PB_STAGE +
-                        (size_t)k8 * (128 * 8) + (size_t)((r & 127) >> 3) * 64 + (r & 7) * 8;
-    *reinterpret_cast<uint4*>(dp) = *reinterpret_cast<uint4*>(p1);
-    *reinterpret_cast<uint4*>(dp + PB_PLANE) = *reinterpret_cast<uint4*>(p2);
-    if constexpr (kPlanes == 3) *reinterpret_cast<uint4*>(dp + 2 * PB_PLANE) = *reinterpret_cast<uint4*>(p3);
     if constexpr (kPlanes == 3)
       *reinterpret_cast<uint4*>(dst + w_tile_off(nt, kc, KC, kPlanes - 1) + off) = *reinterpret_cast<uint4*>(p3);
   }
@@ -1201,7 +720,7 @@ int64_t sr_tc_act_bytes(int64_t M, int K) {
 }
 int64_t sr_tc_weight_bytes(int N, int K) {
   const int64_t NT = (N + sr_tc::BN - 1) / sr_tc::BN, KC = (K + 31) / 32;
-  return 2 * NT * KC * sr_tc::kPlanes * sr_tc::W_PLANE * 2;   // single-CTA layout + CTA-pair layout
+  return NT * KC * sr_tc::kPlanes * sr_tc::W_PLANE * 2;
 }
 
 int sr_tc_pack_rows(const float* src, int64_t M, int K, int ld, void* dst, const int32_t* m_dev,
@@ -1222,100 +741,96 @@ int sr_tc_pack_weights(const float* w, int N, int K, int ld, void* dst, cudaStre
   return sr_launch_status();
 }
 
+static int g_sweep_dbg = 0;
+int sr_tc_debug_sweep_flags(int flags) {
+  const int old = g_sweep_dbg;
+  g_sweep_dbg = flags;
+  return old;
+}
+
+static int tc_fill_step(const sr_tc_step& t, int64_t M, int ch, const int32_t* m_dev, sr_tc::StepArgs& st) {
+  using namespace sr_tc;
+  if (!t.A || !t.W || !t.bias || t.N <= 0 || t.K <= 0 || (!t.A_next && !t.out)) return SR_EINVAL;
+  if (t.mul_tiles && t.mul_K < t.n_valid) return SR_EINVAL;
+  LayerArgs& a = st.la;
+  a.A = (const __nv_bfloat16*)t.A; a.W = (const __nv_bfloat16*)t.W; a.bias = t.bias; a.M = M;
+  a.MT = (int)((M + BM - 1) / BM); a.NT = (t.N + BN - 1) / BN; a.KC = (t.K + 31) / 32;
+  a.n_gemm = t.N; a.n = t.n_valid; a.ch = ch;
+  a.A_next = (__nv_bfloat16*)t.A_next; a.KCn = t.A_next ? (t.K_next + 31) / 32 : 0;
+  a.scale = t.scale; a.skip_src = t.skip_src; a.skip_n = t.skip_n; a.skip_ld = t.skip_ld;
+  a.out = t.out; a.out_ld = t.out_ld; a.dstash = t.dstash; a.out_col0 = t.out_col0; a.out_n = t.out_n;
+  a.mul_tiles = (const __nv_bfloat16*)t.mul_tiles; a.mul_KC = (t.mul_K + 31) / 32;
+  a.mul_inv_scale = t.mul_scale != 0.f ? 1.0f / t.mul_scale : 1.0f; a.m_dev = m_dev;
+  st.mul = t.mul_tiles ? 1 : 0;
+  st.act = t.mul_tiles ? t.mul_act : t.act;
+  return SR_OK;
+}
+
+// picks the instantiation for (body activation, mode, ch) and launches one CTA per row tile, at most one per SM
+static int tc_launch_sweep(sr_tc::SweepArgs& sw, int ch, cudaStream_t s) {
+  using namespace sr_tc;
+  const StepArgs& b = sw.step[0];
+  using Kern = void (*)(const SweepArgs);
+  Kern kern = nullptr;
+#define SR_SW(ACT_, CH_, MUL_) kern = (Kern)tc_sweep_kernel<ACT_, CH_, MUL_>
+  const int key = (ch == 4 ? 10 : 0) + (b.mul ? 5 : 0) + b.act;
+  switch (key) {
+    case 0: SR_SW(SR_ACT_NONE, 1, false); break;
+    case 1: SR_SW(SR_ACT_SOFTPLUS100, 1, false); break;
+    case 2: SR_SW(SR_ACT_RELU, 1, false); break;
+    case 3: SR_SW(SR_ACT_TANH, 1, false); break;
+    case 5: SR_SW(SR_ACT_NONE, 1, true); break;
+    case 6: SR_SW(SR_ACT_SOFTPLUS100, 1, true); break;
+    case 7: SR_SW(SR_ACT_RELU, 1, true); break;
+    case 10: SR_SW(SR_ACT_NONE, 4, false); break;
+    case 11: SR_SW(SR_ACT_SOFTPLUS100, 4, false); break;
+    case 12: SR_SW(SR_ACT_RELU, 4, false); break;
+    case 13: SR_SW(SR_ACT_TANH, 4, false); break;
+    case 15: SR_SW(SR_ACT_NONE, 4, true); break;
+    case 16: SR_SW(SR_ACT_SOFTPLUS100, 4, true); break;
+    case 17: SR_SW(SR_ACT_RELU, 4, true); break;
+  }
+#undef SR_SW
+  if (!kern) return SR_EINVAL;
+  // cudaFuncSetAttribute is per device: one flag per device ordinal (a process may drive several GPUs)
+  static bool attr_set_dev[64][20] = {};
+  int cur_dev = 0;
+  cudaGetDevice(&cur_dev);
+  bool& attr_set = attr_set_dev[cur_dev & 63][key];
+  if (!attr_set) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmem);
+    if (e != cudaSuccess) return (int)e;
+    attr_set = true;
+  }
+  const int MT = b.la.MT;
+  const int grid = MT < SR_NUM_SMS ? MT : SR_NUM_SMS;
+  kern<<<grid, kThreads, kSmem, s>>>(sw);
+  return sr_launch_status();
+}
+
 int sr_tc_linear(const void* A, const void* W, const float* bias, int64_t M, int N, int K, int n_valid,
                  int act, int ch, void* A_next, int K_next, float scale, const float* skip_src,
                  int skip_n, int skip_ld, float* out, int out_ld, int out_col0, int out_n,
                  float* dstash, const void* mul_tiles, int mul_K, int mul_act, float mul_scale,
                  const int32_t* m_dev, cudaStream_t s) {
   using namespace sr_tc;
-  if (!A || !W || !bias || M <= 0 || N <= 0 || K <= 0 || (ch != 1 && ch != 4)) return SR_EINVAL;
-  if (!A_next && !out) return SR_EINVAL;
-  LayerArgs a;
-  a.A = (const __nv_bfloat16*)A; a.W = (const __nv_bfloat16*)W; a.bias = bias; a.M = M;
-  a.MT = (int)((M + BM - 1) / BM); a.NT = (N + BN - 1) / BN; a.KC = (K + 31) / 32;
-  a.Wp = a.W + (size_t)a.NT * a.KC * W_STAGE;
-  a.n_gemm = N; a.n = n_valid; a.ch = ch;
-  a.A_next = (__nv_bfloat16*)A_next; a.KCn = A_next ? (K_next + 31) / 32 : 0;
-  a.scale = scale; a.skip_src = skip_src; a.skip_n = skip_n; a.skip_ld = skip_ld;
-  a.out = out; a.out_ld = out_ld; a.dstash = dstash; a.out_col0 = out_col0; a.out_n = out_n;
-  a.mul_tiles = (const __nv_bfloat16*)mul_tiles; a.mul_KC = (mul_K + 31) / 32;
-  a.mul_inv_scale = mul_scale != 0.f ? 1.0f / mul_scale : 1.0f; a.m_dev = m_dev;
-  if (mul_tiles && mul_K < n_valid) return SR_EINVAL;
-  using Kern = void (*)(const LayerArgs);
-  static const int use_pair = [] { const char* e = getenv("SELFRECON_B200_TC_PAIR"); return e ? atoi(e) : 1; }();
-  // the pair kernel always issues N = 256 MMAs (a narrower N would take columns from BOTH halves)
-  const bool pair = use_pair && a.MT >= 2 && (N % BN == 0);
-#define SR_TC_PICK(ACT_, CH_, MUL_) \
-  (pair ? (Kern)tc_layer_pair_kernel<ACT_, CH_, MUL_> : (Kern)tc_layer_kernel<ACT_, CH_, MUL_>)
-  Kern kern = nullptr;
-  if (mul_tiles && ch == 4) {
-    switch (mul_act) {
-      case SR_ACT_NONE: kern = SR_TC_PICK(SR_ACT_NONE, 4, true); break;
-      case SR_ACT_SOFTPLUS100: kern = SR_TC_PICK(SR_ACT_SOFTPLUS100, 4, true); break;
-      case SR_ACT_RELU: kern = SR_TC_PICK(SR_ACT_RELU, 4, true); break;
-    }
-  } else if (mul_tiles) {
-    switch (mul_act) {
-      case SR_ACT_NONE: kern = SR_TC_PICK(SR_ACT_NONE, 1, true); break;
-      case SR_ACT_SOFTPLUS100: kern = SR_TC_PICK(SR_ACT_SOFTPLUS100, 1, true); break;
-      case SR_ACT_RELU: kern = SR_TC_PICK(SR_ACT_RELU, 1, true); break;
-    }
-  } else if (ch == 1) {
-    switch (act) {
-      case SR_ACT_NONE: kern = SR_TC_PICK(SR_ACT_NONE, 1, false); break;
-      case SR_ACT_SOFTPLUS100: kern = SR_TC_PICK(SR_ACT_SOFTPLUS100, 1, false); break;
-      case SR_ACT_RELU: kern = SR_TC_PICK(SR_ACT_RELU, 1, false); break;
-      case SR_ACT_TANH: kern = SR_TC_PICK(SR_ACT_TANH, 1, false); break;
-    }
-  } else {
-    switch (act) {
-      case SR_ACT_NONE: kern = SR_TC_PICK(SR_ACT_NONE, 4, false); break;
-      case SR_ACT_SOFTPLUS100: kern = SR_TC_PICK(SR_ACT_SOFTPLUS100, 4, false); break;
-      case SR_ACT_RELU: kern = SR_TC_PICK(SR_ACT_RELU, 4, false); break;
-      case SR_ACT_TANH: kern = SR_TC_PICK(SR_ACT_TANH, 4, false); break;
-    }
-  }
-#undef SR_TC_PICK
-  if (!kern) return SR_EINVAL;
-  // cudaFuncSetAttribute is per device: one flag per device ordinal (a process may drive several GPUs)
-  static bool attr_set_dev[64] = {};
-  int cur_dev = 0;
-  cudaGetDevice(&cur_dev);
-  bool& attr_set = attr_set_dev[cur_dev & 63];
-  if (!attr_set) {
-#define SR_TC_BOTH(ACT_, CH_, MUL_)                                                                        \
-  {                                                                                                        \
-    cudaError_t e1 = cudaFuncSetAttribute(tc_layer_kernel<ACT_, CH_, MUL_>,                                \
-                                          cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmem);        \
-    cudaError_t e2 = cudaFuncSetAttribute(tc_layer_pair_kernel<ACT_, CH_, MUL_>,                           \
-                                          cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemPair);    \
-    if (e1 != cudaSuccess) return (int)e1;                                                                 \
-    if (e2 != cudaSuccess) return (int)e2;                                                                 \
-  }
-    SR_TC_BOTH(SR_ACT_NONE, 1, true) SR_TC_BOTH(SR_ACT_SOFTPLUS100, 1, true) SR_TC_BOTH(SR_ACT_RELU, 1, true)
-    SR_TC_BOTH(SR_ACT_NONE, 4, true) SR_TC_BOTH(SR_ACT_SOFTPLUS100, 4, true) SR_TC_BOTH(SR_ACT_RELU, 4, true)
-    SR_TC_BOTH(SR_ACT_NONE, 1, false) SR_TC_BOTH(SR_ACT_SOFTPLUS100, 1, false) SR_TC_BOTH(SR_ACT_RELU, 1, false)
-    SR_TC_BOTH(SR_ACT_TANH, 1, false) SR_TC_BOTH(SR_ACT_NONE, 4, false) SR_TC_BOTH(SR_ACT_SOFTPLUS100, 4, false)
-    SR_TC_BOTH(SR_ACT_RELU, 4, false) SR_TC_BOTH(SR_ACT_TANH, 4, false)
-#undef SR_TC_BOTH
-    attr_set = true;
-  }
-  if (pair) {
-    const long long npt = (long long)((a.MT + 1) / 2) * a.NT;
-    const long long npairs = npt < SR_NUM_SMS_B200 / 2 ? npt : SR_NUM_SMS_B200 / 2;
-    kern<<<(unsigned)(2 * npairs), epi_threads(mul_tiles != nullptr), kSmemPair, s>>>(a);
-  } else {
-    const long long ntiles = (long long)a.MT * a.NT;
-    const int grid = (int)(ntiles < SR_NUM_SMS_B200 ? ntiles : SR_NUM_SMS_B200);
-    kern<<<grid, epi_threads(mul_tiles != nullptr), kSmem, s>>>(a);
-  }
-  return sr_launch_status();
-}
-static int g_sweep_dbg = 0;
-int sr_tc_debug_sweep_flags(int flags) {
-  const int old = g_sweep_dbg;
-  g_sweep_dbg = flags;
-  return old;
+  if (M <= 0 || (ch != 1 && ch != 4)) return SR_EINVAL;
+  sr_tc_step t = {};
+  t.A = A; t.W = W; t.bias = bias; t.A_next = A_next; t.skip_src = skip_src; t.out = out;
+  t.mul_tiles = mul_tiles; t.dstash = dstash;
+  t.N = N; t.K = K; t.n_valid = n_valid; t.act = act; t.K_next = K_next; t.skip_n = skip_n; t.skip_ld = skip_ld;
+  t.out_ld = out_ld; t.out_col0 = out_col0; t.out_n = out_n; t.mul_K = mul_K; t.mul_act = mul_act;
+  t.scale = scale; t.mul_scale = mul_scale;
+  if (mul_tiles ? (mul_act != SR_ACT_NONE && mul_act != SR_ACT_SOFTPLUS100 && mul_act != SR_ACT_RELU)
+                : (act < SR_ACT_NONE || act > SR_ACT_TANH))
+    return SR_EINVAL;
+  SweepArgs sw;
+  sw.L = 1;
+  sw.dbg = 0;
+  sw.last_plain = 0;
+  const int rc = tc_fill_step(t, M, ch, m_dev, sw.step[0]);
+  if (rc) return rc;
+  return tc_launch_sweep(sw, ch, s);
 }
 
 int sr_tc_sweep(const sr_tc_step* steps, int L, int64_t M, int ch, const int32_t* m_dev, cudaStream_t s) {
@@ -1324,28 +839,15 @@ int sr_tc_sweep(const sr_tc_step* steps, int L, int64_t M, int ch, const int32_t
   SweepArgs sw;
   sw.L = L;
   sw.dbg = g_sweep_dbg;
-  const int MT = (int)((M + BM - 1) / BM);
   for (int l = 0; l < L; ++l) {
     const sr_tc_step& t = steps[l];
-    if (!t.A || !t.W || !t.bias || t.N <= 0 || t.K <= 0 || (!t.A_next && !t.out)) return SR_EINVAL;
     if (t.act != SR_ACT_NONE && t.act != SR_ACT_SOFTPLUS100 && t.act != SR_ACT_RELU) return SR_EINVAL;
     if (t.mul_tiles && (t.mul_act != SR_ACT_NONE && t.mul_act != SR_ACT_SOFTPLUS100 && t.mul_act != SR_ACT_RELU))
       return SR_EINVAL;
-    if (t.mul_tiles && t.mul_K < t.n_valid) return SR_EINVAL;
-    LayerArgs& a = sw.step[l].la;
-    a.A = (const __nv_bfloat16*)t.A; a.W = (const __nv_bfloat16*)t.W; a.bias = t.bias; a.M = M;
-    a.MT = MT; a.NT = (t.N + BN - 1) / BN; a.KC = (t.K + 31) / 32;
-    a.Wp = a.W + (size_t)a.NT * a.KC * W_STAGE;
-    a.n_gemm = t.N; a.n = t.n_valid; a.ch = ch;
-    a.A_next = (__nv_bfloat16*)t.A_next; a.KCn = t.A_next ? (t.K_next + 31) / 32 : 0;
-    a.scale = t.scale; a.skip_src = t.skip_src; a.skip_n = t.skip_n; a.skip_ld = t.skip_ld;
-    a.out = t.out; a.out_ld = t.out_ld; a.dstash = t.dstash; a.out_col0 = t.out_col0; a.out_n = t.out_n;
-    a.mul_tiles = (const __nv_bfloat16*)t.mul_tiles; a.mul_KC = (t.mul_K + 31) / 32;
-    a.mul_inv_scale = t.mul_scale != 0.f ? 1.0f / t.mul_scale : 1.0f; a.m_dev = m_dev;
-    sw.step[l].mul = t.mul_tiles ? 1 : 0;
-    sw.step[l].act = t.mul_tiles ? t.mul_act : t.act;
+    const int rc = tc_fill_step(t, M, ch, m_dev, sw.step[l]);
+    if (rc) return rc;
   }
-  // one buffer, two tile widths: the layouts alias across row tiles, and pairs run through the steps unsynchronised
+  // one buffer, two tile widths: the layouts alias across row tiles, and CTAs run through the steps unsynchronised
   for (int i = 0; i < L; ++i)
     for (int j = 0; j < L; ++j) {
       const LayerArgs &x = sw.step[i].la, &y = sw.step[j].la;
@@ -1356,41 +858,9 @@ int sr_tc_sweep(const sr_tc_step* steps, int L, int64_t M, int ch, const int32_t
   // every step but an optional plain last one shares (activation, mode)
   const int body_act = sw.step[0].act, body_mul = sw.step[0].mul;
   const StepArgs& lastp = sw.step[L - 1];
-  sw.last_plain = (L > 1 || true) && !lastp.mul && lastp.act == SR_ACT_NONE && (body_mul || body_act != SR_ACT_NONE) ? 1 : 0;
+  sw.last_plain = !lastp.mul && lastp.act == SR_ACT_NONE && (body_mul || body_act != SR_ACT_NONE) ? 1 : 0;
   for (int l = 0; l < L - (sw.last_plain ? 1 : 0); ++l)
     if (sw.step[l].act != body_act || sw.step[l].mul != body_mul) return SR_EINVAL;
-  using Kern = void (*)(const SweepArgs);
-  Kern kern = nullptr;
-#define SR_SW(ACT_, CH_, MUL_) kern = (Kern)tc_sweep_pair_kernel<ACT_, CH_, MUL_>
-  const int key = (ch == 4 ? 8 : 0) + (body_mul ? 4 : 0) + body_act;
-  switch (key) {
-    case 0: SR_SW(SR_ACT_NONE, 1, false); break;
-    case 1: SR_SW(SR_ACT_SOFTPLUS100, 1, false); break;
-    case 2: SR_SW(SR_ACT_RELU, 1, false); break;
-    case 4: SR_SW(SR_ACT_NONE, 1, true); break;
-    case 5: SR_SW(SR_ACT_SOFTPLUS100, 1, true); break;
-    case 6: SR_SW(SR_ACT_RELU, 1, true); break;
-    case 8: SR_SW(SR_ACT_NONE, 4, false); break;
-    case 9: SR_SW(SR_ACT_SOFTPLUS100, 4, false); break;
-    case 10: SR_SW(SR_ACT_RELU, 4, false); break;
-    case 12: SR_SW(SR_ACT_NONE, 4, true); break;
-    case 13: SR_SW(SR_ACT_SOFTPLUS100, 4, true); break;
-    case 14: SR_SW(SR_ACT_RELU, 4, true); break;
-  }
-#undef SR_SW
-  if (!kern) return SR_EINVAL;
-  static bool attr_set_dev[64][16] = {};
-  int cur_dev = 0;
-  cudaGetDevice(&cur_dev);
-  bool& attr_set = attr_set_dev[cur_dev & 63][key];
-  if (!attr_set) {
-    cudaError_t e1 = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemPair);
-    if (e1 != cudaSuccess) return (int)e1;
-    attr_set = true;
-  }
-  const int nrp = (MT + 1) / 2;
-  const int npairs = nrp < SR_NUM_SMS_B200 / 2 ? nrp : SR_NUM_SMS_B200 / 2;
-  kern<<<(unsigned)(2 * npairs), epi_threads(body_mul != 0), kSmemPair, s>>>(sw);
-  return sr_launch_status();
+  return tc_launch_sweep(sw, ch, s);
 }
 }

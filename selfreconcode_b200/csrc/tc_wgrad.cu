@@ -6,20 +6,20 @@
 // Both operands already exist as tiled split-bf16 activations (tc_common.cuh): `x` = the layer's input tiles
 // the forward sweep kept, `delta` = the cotangent tiles the reverse sweep wrote.  In that layout a core matrix
 // is 8 rows x 8 features with the FEATURES contiguous, which is exactly the canonical MN-major core matrix of
-// a UMMA operand whose GEMM-K dimension is the ROW index -- so the same bytes feed this GEMM with
-// a_major = b_major = MN and no transposition pass:
-//      D[128 delta-features x N x-features] += A^T[128 x 16 rows] * B[16 rows x N]      (N <= 256)
-// per `tcgen05.mma.cta_group::1.kind::f16`, 3 MMAs per product (split-bf16 cross terms, as in tc_gemm.cu).
+// a wgmma operand whose GEMM-K dimension is the ROW index -- so the same bytes feed this GEMM as transposed
+// (MN-major) A and B operands and no transposition pass is needed:
+//      D[64 delta-features x 256 x-features] += A^T[64 x 16 rows] * B[16 rows x 256]
+// per `wgmma.mma_async m64n256k16` and warpgroup, 3 MMAs per product (split-bf16 cross terms, as in tc_gemm.cu).
 //
 // One CTA owns one (128 x 256) tile of dW and a contiguous range of row half-tiles (split-K over points):
-//   warp 0      TMA producer: a stage = 64 rows; per stage 32 + 64 bulk copies of 1 KB (one k8 group of one
-//               plane each) land the planes of 128 + 256 features separately, so that the feature stride is
-//               uniform (SBO = 1 KB, LBO = 128 B); the 32 lanes issue the copies in parallel
-//   warp 1      MMA issuer (one thread); switches between two 256-column TMEM accumulators every kFlush stages
-//   warps 2..5  drain the idle accumulator and add it to the CTA's fp32 partial tile in global memory with plain
-//               read-modify-write (each element is always handled by the same thread: deterministic).  Bounding
-//               the run length of an accumulator bounds the truncation bias of the tensor core's fp32 adder
-//               (tc_gemm.cu header): 16 stages = 1024 rows = 192 accumulations per element.
+//   warp 0          TMA producer: a stage = 64 rows; per stage 32 + 64 bulk copies of 1 KB (one k8 group of one
+//                   plane each) land the planes of 128 + 256 features separately, so that the feature stride is
+//                   uniform (SBO = 1 KB, LBO = 128 B); the 32 lanes issue the copies in parallel
+//   warpgroups 1-2  delta features [0, 64) / [64, 128) of the tile: MMAs into registers; every kFlush stages the
+//                   accumulator is added to the CTA's fp32 partial tile in global memory with plain
+//                   read-modify-write (each element is always handled by the same thread: deterministic).  Bounding
+//                   the run length of an accumulator bounds the truncation bias of the tensor core's fp32 adder
+//                   (tc_gemm.cu header): 16 stages = 1024 rows = 192 accumulations per element.
 // A second kernel adds the split partials in a fixed order into dW (row-major [n][k], nn.Linear.weight's layout).
 // The bias gradient (column sums of delta over VALUE rows) is a separate streaming kernel.
 #include <cstdlib>
@@ -35,7 +35,8 @@ constexpr int WG_B_PLANE_BYTES = 32 * 1024;         // 256 features x 64 rows x 
 constexpr int WG_STAGE_BYTES = kPlanes * (WG_A_PLANE_BYTES + WG_B_PLANE_BYTES);   // 96 KB
 constexpr size_t kSmemWgrad = (size_t)WG_STAGES * WG_STAGE_BYTES + 256;
 constexpr int kFlush = 16;                          // stages per accumulator run
-constexpr int kWgThreads = 64 + 4 * 32;
+constexpr int kWgThreads = 3 * 128;
+constexpr int kWgConsumerWarps = 8;
 static_assert(kPlanes == 2, "the weight-gradient kernel is written for 2 planes / 3 terms");
 
 struct WgradArgs {
@@ -48,38 +49,42 @@ struct WgradArgs {
   int desc_swap;            // debugging aid: swap the LBO / SBO fields of the descriptors
 };
 
+// one stage (64 rows) of this warpgroup's 64 x 256 accumulator: 3 terms x 4 row steps of 16
+template <bool FIRST>
+__device__ __forceinline__ void wgrad_stage(float (&acc)[128], uint32_t abase, uint32_t bbase, uint32_t lbo,
+                                            uint32_t sbo) {
+  const int pa[3] = {0, 1, 0}, pb[3] = {1, 0, 0};   // smallest contributions first
+#pragma unroll
+  for (int q = 0; q < 3; ++q) {
+#pragma unroll
+    for (int j = 0; j < WG_ROWS / 16; ++j) {
+      const uint64_t ad = make_desc(abase + pa[q] * WG_A_PLANE_BYTES + j * 256, lbo, sbo);
+      const uint64_t bd = make_desc(bbase + pb[q] * WG_B_PLANE_BYTES + j * 256, lbo, sbo);
+      if (FIRST && q == 0 && j == 0) wgmma_m64n256k16<1, 1, true>(acc, ad, bd);
+      else wgmma_m64n256k16<1, 1, false>(acc, ad, bd);
+    }
+  }
+}
+
 __global__ void __launch_bounds__(kWgThreads, 1) tc_wgrad_kernel(const __grid_constant__ WgradArgs a) {
   extern __shared__ __align__(1024) unsigned char smem[];
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)WG_STAGES * WG_STAGE_BYTES);
   uint64_t* full = bars;                  // [WG_STAGES]
   uint64_t* empty = bars + WG_STAGES;     // [WG_STAGES]
-  uint64_t* tfull = bars + 2 * WG_STAGES; // [2]
-  uint64_t* tempty = tfull + 2;           // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7;
   if (threadIdx.x == 0) {
-    for (int i = 0; i < WG_STAGES; ++i) { sr_mbar_init(&full[i], 1); sr_mbar_init(&empty[i], 1); }
-    for (int i = 0; i < 2; ++i) { sr_mbar_init(&tfull[i], 1); sr_mbar_init(&tempty[i], 4); }
+    for (int i = 0; i < WG_STAGES; ++i) { sr_mbar_init(&full[i], 1); sr_mbar_init(&empty[i], kWgConsumerWarps); }
     sr_fence_barrier_init();
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(sr_smem_u32(tmem_slot)),
-                 "r"(512)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   const int tile = blockIdx.x / a.splits, split = blockIdx.x % a.splits;
   const int tm = tile / a.tiles_n, tn = tile % a.tiles_n;
-  const int nb = min(8, a.KCx - tn * 8);              // 32-feature chunks of x in this tile (MMA N = 32 nb)
-  const int na = min(4, a.KCd - tm * 4);              // 32-feature chunks of delta in this tile; a short last tile
-                                                      // leaves stale shared memory in the other rows of the M = 128
-                                                      // operand: those accumulator rows are simply never stored
+  const int nb = min(8, a.KCx - tn * 8);              // 32-feature chunks of x in this tile; the MMA always runs
+                                                      // N = 256: columns past 32 nb see stale shared memory and are
+                                                      // never stored
+  const int na = min(4, a.KCd - tm * 4);              // 32-feature chunks of delta in this tile (same for rows)
   const int halves = 2 * a.MT;
   const int per = (halves + a.splits - 1) / a.splits;
   const int h0 = split * per, h1 = min(halves, h0 + per);
@@ -118,87 +123,64 @@ __global__ void __launch_bounds__(kWgThreads, 1) tc_wgrad_kernel(const __grid_co
       }
       if (++slot == WG_STAGES) { slot = 0; phase ^= 1u; }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer
-    if (lane == 0) {
-      int slot = 0;
-      uint32_t phase = 0;
-      // D = f32, A = B = bf16, both MN-major (bits 15, 16), M = 128, N = 32 nb
-      const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (1u << 16) |
-                             ((uint32_t)((32 * nb) >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-      const uint32_t lbo = a.desc_swap ? 1024u : 128u, sbo = a.desc_swap ? 128u : 1024u;
-      const int pa[3] = {0, 1, 0}, pb[3] = {1, 0, 0};   // smallest contributions first
-      int s = 0;
-      for (int run = 0; run < nruns; ++run) {
-        const int buf = run & 1;
-        sr_mbar_wait(&tempty[buf], ((run >> 1) & 1) ^ 1u);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + (uint32_t)buf * 256;
-        uint32_t accumulate = 0;
-        const int s_end = min(nstages, s + kFlush);
-        for (; s < s_end; ++s) {
-          sr_mbar_wait(&full[slot], phase);
-          tc_fence_after();
-          const uint32_t abase = sr_smem_u32(smem + (size_t)slot * WG_STAGE_BYTES);
-          const uint32_t bbase = abase + kPlanes * WG_A_PLANE_BYTES;
-#pragma unroll
-          for (int q = 0; q < 3; ++q) {
-#pragma unroll
-            for (int j = 0; j < WG_ROWS / 16; ++j) {
-              const uint64_t ad = make_desc(abase + pa[q] * WG_A_PLANE_BYTES + j * 256, lbo, sbo);
-              const uint64_t bd = make_desc(bbase + pb[q] * WG_B_PLANE_BYTES + j * 256, lbo, sbo);
-              mma_bf16(tmem_d, ad, bd, idesc, accumulate);
-              accumulate = 1;
-            }
-          }
-          mma_commit(&empty[slot]);
-          if (++slot == WG_STAGES) { slot = 0; phase ^= 1u; }
-        }
-        mma_commit(&tfull[buf]);
-      }
-    }
-  } else {
-    // ------------------------------------------------------------------ drain (warps 2..5)
-    const int q = warp & 3;                               // TMEM lane quarter of this warp
-    const int row = tm * 128 + q * 32 + lane;             // delta feature
-    const bool row_ok = row < a.KCd * 32;
+  } else if (wg > 0) {
+    // ------------------------------------------------------------------ MMA + drain (warpgroups 1, 2)
+    const int cw = wg - 1, wq = warp & 3;
+    const uint32_t lbo = a.desc_swap ? 1024u : 128u, sbo = a.desc_swap ? 128u : 1024u;
+    // fragment rows (delta features) 16 wq + lane / 4 (+ 8) of this warpgroup's 64, columns 8 i + 2 (lane % 4) (+ 1)
+    const int row0 = tm * 128 + cw * 64 + 16 * wq + (lane >> 2);
     const size_t ld = (size_t)a.KCx * 32;
-    float* dst = a.part + ((size_t)split * ((size_t)a.KCd * 32) + row) * ld + (size_t)tn * 256;
+    float* dst0 = a.part + ((size_t)split * ((size_t)a.KCd * 32) + row0) * ld + (size_t)tn * 256 + 2 * (lane & 3);
+    const bool ok0 = row0 < a.KCd * 32, ok1 = row0 + 8 < a.KCd * 32;
+    const int ncols8 = 4 * nb;                        // stored 8-column blocks
+    float acc[128];
+    int slot = 0;
+    uint32_t phase = 0;
+    int s = 0;
+    // operands of stage `slot`: this warpgroup's 64 delta features (8 groups of 8) and the 256 x features
+    auto abase = [&](int sl) { return sr_smem_u32(smem + (size_t)sl * WG_STAGE_BYTES) + cw * 8 * 1024; };
+    auto bbase = [&](int sl) { return sr_smem_u32(smem + (size_t)sl * WG_STAGE_BYTES) + kPlanes * WG_A_PLANE_BYTES; };
     for (int run = 0; run < nruns; ++run) {
-      const int buf = run & 1;
-      sr_mbar_wait(&tfull[buf], (run >> 1) & 1);
-      tc_fence_after();
-      const uint32_t taddr0 = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)buf * 256;
-      for (int c = 0; c < nb; ++c) {
-        uint32_t v[32];
-        tmem_ld32_async(taddr0 + c * 32, v);
-        tmem_wait(v);
-        if (!row_ok) continue;
-        float4* d4 = reinterpret_cast<float4*>(dst + c * 32);
-#pragma unroll
-        for (int j4 = 0; j4 < 8; ++j4) {
-          float4 o = make_float4(__uint_as_float(v[4 * j4]), __uint_as_float(v[4 * j4 + 1]),
-                                 __uint_as_float(v[4 * j4 + 2]), __uint_as_float(v[4 * j4 + 3]));
-          if (run > 0) {
-            const float4 old = d4[j4];
-            o.x += old.x; o.y += old.y; o.z += old.z; o.w += old.w;
-          }
-          d4[j4] = o;
-        }
+      const int s_end = min(nstages, s + kFlush);
+      // the first stage of a run overwrites the accumulator (peeled: no data-dependent branch around the MMAs)
+      sr_mbar_wait(&full[slot], phase);
+      wgmma_fence();
+      wgrad_stage<true>(acc, abase(slot), bbase(slot), lbo, sbo);
+      wgmma_commit();
+      int prev = slot;
+      if (++slot == WG_STAGES) { slot = 0; phase ^= 1u; }
+      for (++s; s < s_end; ++s) {
+        sr_mbar_wait(&full[slot], phase);
+        wgmma_fence();
+        wgrad_stage<false>(acc, abase(slot), bbase(slot), lbo, sbo);
+        wgmma_commit();
+        wgmma_wait<1>();   // the previous stage's MMAs are complete: release it
+        if (lane == 0) sr_mbar_arrive(&empty[prev]);
+        prev = slot;
+        if (++slot == WG_STAGES) { slot = 0; phase ^= 1u; }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) sr_mbar_arrive(&tempty[buf]);
+      wgmma_wait<0>();
+      if (lane == 0) sr_mbar_arrive(&empty[prev]);
+#pragma unroll
+      for (int i = 0; i < 32; ++i) {
+        if (i >= ncols8) break;
+        float2 o0 = make_float2(acc[4 * i], acc[4 * i + 1]), o1 = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
+        float2* d0 = reinterpret_cast<float2*>(dst0 + 8 * i);
+        float2* d1 = reinterpret_cast<float2*>(dst0 + 8 * ld + 8 * i);
+        if (run > 0) {
+          if (ok0) { const float2 t = *d0; o0.x += t.x; o0.y += t.y; }
+          if (ok1) { const float2 t = *d1; o1.x += t.x; o1.y += t.y; }
+        }
+        if (ok0) *d0 = o0;
+        if (ok1) *d1 = o1;
+      }
     }
-    if (nruns == 0 && row_ok) {   // a split without rows still owns its partial tile
-      for (int c = 0; c < nb * 8; ++c) reinterpret_cast<float4*>(dst)[c] = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (nruns == 0) {   // a split without rows still owns its partial tile
+      for (int i = 0; i < ncols8; ++i) {
+        if (ok0) *reinterpret_cast<float2*>(dst0 + 8 * i) = make_float2(0.f, 0.f);
+        if (ok1) *reinterpret_cast<float2*>(dst0 + 8 * ld + 8 * i) = make_float2(0.f, 0.f);
+      }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
   }
 }
 
@@ -273,7 +255,7 @@ int64_t sr_tc_wgrad_partial_bytes(int64_t M, int Kd, int Kx, int* splits_out) {
   using namespace sr_tc;
   const int MT = (int)((M + BM - 1) / BM), KCd = (Kd + 31) / 32, KCx = (Kx + 31) / 32;
   const int tiles = ((KCd + 3) / 4) * ((KCx + 7) / 8);
-  int splits = SR_NUM_SMS_B200 / (tiles > 0 ? tiles : 1);
+  int splits = SR_NUM_SMS / (tiles > 0 ? tiles : 1);
   if (splits < 1) splits = 1;
   if (splits > 2 * MT) splits = 2 * MT;
   if (splits_out) *splits_out = splits;

@@ -1,5 +1,5 @@
 // Pointwise stages of the tensor-core tracer (OptimizeSurfacePs, utils/FindSurfacePs.py:114-163).
-// The dense layers run as tcgen05 split-BF16 GEMM launches (tc_gemm.cu); between them two small
+// The dense layers run as wgmma split-BF16 GEMM launches (tc_gemm.cu); between them two small
 // kernels do everything that is per-ray:
 //   trace_mid    after the forward sweeps: LBS of p + offset (warp per ray), convergence test,
 //                loss, and the cotangents that seed the two backward sweeps

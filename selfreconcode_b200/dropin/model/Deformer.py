@@ -1,5 +1,5 @@
 """Non-rigid deformation field: MLP offset + SMPL linear-blend skinning
-(reference: model/Deformer.py:10-233) on the fused B200 engine.
+(reference: model/Deformer.py:10-233) on the fused CUDA engines.
 
 Class names, constructor signatures, buffers and state_dict keys follow the reference
 (`defs.0.lin{l}.weight/bias`, `defs.1.{b_min,b_max,ws,Js,init_pose}`).  Without autograd the

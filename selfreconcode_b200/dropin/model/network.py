@@ -1,4 +1,4 @@
-"""Neural SDF (reference: model/network.py:14-118) on the fused B200 engine.
+"""Neural SDF (reference: model/network.py:14-118) on the fused CUDA engines.
 
 `ImplicitNetwork` keeps the reference's constructor signature, initialisation, attribute names
 and state_dict keys (lin{l}.weight_g / weight_v / bias), and the `rendcond` side effect of
@@ -110,7 +110,7 @@ class ImplicitNetwork(nn.Module):
         pts = input.detach().reshape(-1, 3)
         if ops.TC_ENABLED and not want_grad and nfeat == 0 and pts.shape[0] >= ops.TC_MIN_POINTS:
             # large value-only batches (the 257^3 / 513^3 grid queries): tensor-core engine
-            # (tcgen05 split-BF16 GEMM per layer, csrc/tc_gemm.cu)
+            # (wgmma split-BF16 GEMM per layer, csrc/tc_gemm.cu)
             sdf = ops.tc_mlp_forward(net, pts, ch=1, n_out=1)
             if refine_about is not None and ops.TC_REFINE:
                 ops.sdf_refine_band(net, pts.contiguous().float(), sdf.view(-1), float(refine_about))

@@ -17,21 +17,19 @@ from ._lib import check as _check
 
 import os as _os
 
-# Tensor-core engine switch: large batches go to the tcgen05 split-BF16 layer GEMMs, small ones to the
+# Tensor-core engine switch: large batches go to the wgmma split-BF16 layer GEMMs, small ones to the
 # fused fp32 FFMA engine (one persistent kernel, lower latency).  SELFRECON_B200_TC=0 disables it.
 TC_ENABLED = _os.environ.get("SELFRECON_B200_TC", "1") != "0"
-# 2048: at the reference's real per-step batch (~6 144 rays, config.conf:3,113) a tensor-core trace is launch bound
-# (~4 ms, or one graph replay) while the fp32 engine needs ~20 ms
+# 2048: below it a tensor-core trace is launch bound and the fp32 engine (one persistent kernel) is the faster choice
 TC_MIN_POINTS = int(_os.environ.get("SELFRECON_B200_TC_MIN_POINTS", "2048"))
 
 # Borderline decisions on tensor-core values are re-taken on the fp32 FFMA engine (DESIGN.md section 4):
-# TC_EPS_F bounds the engine's absolute error on an SDF value (measured 2.4e-5 against fp64, csrc/tc_gemm.cu),
+# TC_EPS_F bounds the engine's absolute error on an SDF value (split-BF16 with fp32 accumulation, csrc/tc_gemm.cu),
 # TC_EPS_A (degrees) the error of the ray/point angle that follows from D(p)'s.
 TC_EPS_F = float(_os.environ.get("SELFRECON_B200_TC_EPS_F", "4e-5"))
 TC_EPS_A = float(_os.environ.get("SELFRECON_B200_TC_EPS_A", "1e-3"))
 TC_REFINE = _os.environ.get("SELFRECON_B200_TC_REFINE", "1") != "0"
-# The tracer's in-loop fp32 re-test costs one latency-bound FFMA launch per iteration (~1.2 ms each at the bench
-# size) and cannot remove the dominant source of per-ray divergence (sign(f) in the update when |f| is below the
+# The tracer's in-loop fp32 re-test costs one latency-bound FFMA launch per iteration and cannot remove the dominant source of per-ray divergence (sign(f) in the update when |f| is below the
 # engine's error, DESIGN.md section 4): off by default, kept for experiments.
 TC_REFINE_TRACE = _os.environ.get("SELFRECON_B200_TC_REFINE_TRACE", "0") != "0"
 TC_DUAL_STREAM = _os.environ.get("SELFRECON_B200_TC_DUAL_STREAM", "1") != "0"
@@ -478,7 +476,7 @@ def sdf_refine_band(net, pts, sdf, center=0.0, eps=None):
         cnt.zero_()
         check(lib.sr_band_select(_p(sdf), P, float(center), eps, _p(lst), _p(cnt), _stream()), "band_select")
         if SMALL_REFINE:
-            # short lists: one column-split launch per layer (~0.1 ms) instead of the persistent engine (~1 ms per tile);
+            # short lists: one column-split launch per layer instead of the persistent engine's per-tile latency;
             # the list is longer than SMALL_CAP only in degenerate cases -- then the persistent engine takes all of it
             wkey = key + ("small",)
             work = _band_scratch.get(wkey)
@@ -624,7 +622,7 @@ def trace_surface_points(sdf_net, def_net, lbs, cam_pos, rays, init_pts, batch_i
                          dthreshold=5e-5, athreshold=0.02, w1=3.05, w2=1.0, times=5,
                          return_counters=False, mode="auto"):
     """OptimizeSurfacePs (utils/FindSurfacePs.py:114-163): returns (points, converged).
-    Nothing syncs the host.  mode: "tc" = dense layers on the tensor-core engine (tcgen05 split-BF16,
+    Nothing syncs the host.  mode: "tc" = dense layers on the tensor-core engine (wgmma split-BF16,
     reverse-mode sweeps), "reverse" / "forward" = fused fp32 FFMA engine (times+1 launches of one
     persistent kernel), "auto" = "tc" for large ray sets, "reverse" otherwise."""
     if mode == "auto":
@@ -750,7 +748,7 @@ def seg3d_scatter(lin, values, interp, balance, grid_flat):
 
 
 # ------------------------------------------------------------------------------------------------
-# Tensor-core (tcgen05, split-BF16) layer engine
+# Tensor-core (wgmma, split-BF16) layer engine
 # ------------------------------------------------------------------------------------------------
 def tc_pack_rows(x):
     """fp32 [M,K] -> tiled split-bf16 activation buffer (uint8 tensor)."""
@@ -765,7 +763,7 @@ def tc_pack_rows(x):
 
 
 def tc_pack_weights(w):
-    """effective weights fp32 [N,K] -> tiled split-bf16 weight buffer (single-CTA + CTA-pair layouts) (uint8 tensor)."""
+    """effective weights fp32 [N,K] -> tiled split-bf16 weight buffer (uint8 tensor)."""
     _need_cuda(w)
     w = w.contiguous().float()
     N, K = w.shape
@@ -839,7 +837,7 @@ def tc_net(fused):
     return t
 
 
-TC_SWEEP = _os.environ.get("SELFRECON_B200_TC_SWEEP", "0") != "0"   # measured slower than per-layer launches (DESIGN 3.1b)
+TC_SWEEP = _os.environ.get("SELFRECON_B200_TC_SWEEP", "0") != "0"   # off by default: one launch per layer
 _SWEEP_ACTS = (0, 1, 2)      # SR_ACT_NONE / SOFTPLUS100 / RELU: what the whole-sweep kernel's epilogues cover
 _STEP_DEFAULTS = dict(A_next=None, K_next=0, scale=1.0, skip_src=None, skip_n=0, skip_ld=0, out=None, out_ld=0,
                       out_col0=0, out_n=0, dstash=None, mul_tiles=None, mul_K=0, mul_act=0, mul_scale=1.0)
@@ -888,7 +886,7 @@ def _run_steps(lib, steps, M, ch, m_dev):
 
 def tc_mlp_forward(fused, pts, ch=1, conds=None, batch_inds=None, pts_per_frame=0, n_out=None,
                    want_dstash=False):
-    """Whole MLP on the tensor-core engine: embed -> pack -> one tcgen05 launch per layer.
+    """Whole MLP on the tensor-core engine: embed -> pack -> one wgmma launch per layer.
     Returns out fp32 [P*ch, n_out] (last-layer outputs; tangent rows hold d out / d p_t)."""
     _need_cuda(pts)
     net = tc_net(fused)

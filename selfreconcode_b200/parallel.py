@@ -1,6 +1,6 @@
 """One-process-per-GPU data parallelism for the hot path (SURVEY.md section 8e).
 
-The reference has no distributed code at all; this is the B200-native design:
+The reference has no distributed code at all; this is the native design:
 
   * training  : frames (and their rays) are sharded across ranks; every rank holds full replicas
                 of the three MLPs, the skin volume and the template mesh.  Gradients reach .grad

@@ -12,8 +12,8 @@ network (it contains act''), which is exactly what `loss.backward()` over a `cre
         x0  [M, ld]  fp32 embedded input rows (M = points * ch; ch = 4: value row then three tangent rows; ch = 1)
         W_l [n, k]   effective weights (weight norm already applied by differentiable torch ops outside)
         out [M, n_last]
-    forward : pack -> sr_tc_linear per layer (tcgen05 split-bf16, activations kept as tiles)
-    backward: pack cotangents -> per layer  sr_tc_wgrad (dW = delta^T x, MN-major tcgen05 GEMM over the kept tiles),
+    forward : pack -> sr_tc_linear per layer (wgmma split-bf16, activations kept as tiles)
+    backward: pack cotangents -> per layer  sr_tc_wgrad (dW = delta^T x, MN-major wgmma GEMM over the kept tiles),
               sr_tc_colsum (db), sr_tc_linear reverse launch (delta_{l-1}; ch = 4 epilogue couples the rows)
 No cuBLAS, no torch matmul: torch only carries memory, the embedding and the pointwise loss arithmetic.
 """
@@ -378,9 +378,8 @@ class WeightNormAllFunction(torch.autograd.Function):
 
 import os as _os
 
-# Off by default: parity-tested (tests/test_gpu_train.py) and 360 launches fewer per optimisation step, but in the one
-# bench run it was on, the optimizer phase of the step grew from 0.8 to 7.1 ms (forward / backward / propagate shrank by
-# 0.8 / 1.0 / 1.2 ms) and the GPU budget of the round ended before that could be bisected (DESIGN.md 7c).
+# Off by default: parity-tested (tests/test_gpu_train.py) and 360 launches fewer per optimisation step, but the one
+# bench run with it on showed a slower optimizer phase that was never bisected (DESIGN.md section 8).
 FUSED_WEIGHT_NORM = _os.environ.get("SELFRECON_B200_FUSED_WN", "0") != "0"
 
 

@@ -1,9 +1,9 @@
-"""GPU parity tests (run on the B200 box: `pytest -m gpu`).
+"""GPU parity tests (`pytest -m gpu`, on an H100).
 
 Every test calls the product through its C-ABI wrappers / drop-in modules and compares with
   (1) the golden vectors recorded from the unmodified reference (tests/golden/),
   (2) the CPU oracle on the same seeded inputs,
-  (3) where built, the reference's own CUDA kernels from oracle/_ref/ (A/B on the same GPU).
+  (3) what the reference's own CUDA kernels computed on the same inputs (tests/golden/ref_kernels.npz).
 Bars: bit-exact for integer / index work (MC faces and vertex ids, sampler corner indices,
 masks away from thresholds, boundary flags); 1e-4 norm-wise relative for floating point
 (the north star's tolerance), tighter where the arithmetic allows it.
@@ -18,16 +18,6 @@ from helpers import (RATIO, SMPL_PARENTS, build_render, build_sdf_full, build_sd
 
 pytestmark = pytest.mark.gpu
 FP_TOL = 1e-4
-
-
-def helpers_root():
-    import helpers
-    return helpers.ROOT
-
-
-def _ref(name):
-    from oracle import build
-    return build.load_ref(name)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -72,16 +62,23 @@ def test_minv3x3_forward_backward(cuda_dev):
     assert inv0.shape == (0, 3, 3) and chk0.shape == (0,)
 
 
+# The *_matches_reference_kernel tests compare with what the reference's own CUDA extensions computed on the same
+# seeded inputs (tests/golden/ref_kernels.npz, written by oracle/make_golden_ref_kernels.py).
+MINV_REF_N = 2048   # matrices stored (the inputs are drawn for 8192)
+
+
+def _minv_inputs():
+    g = torch.Generator().manual_seed(1)
+    return torch.randn(8192, 3, 3, generator=g), torch.randn(8192, 3, 3, generator=g)
+
+
 def test_minv3x3_matches_reference_kernel(cuda_dev):
-    ref = _ref("FastMinv")
-    if ref is None:
-        pytest.skip("oracle/_ref/FastMinv.so not built")
+    ref = golden("ref_kernels.npz")
     dropin()
     import FastMinv
-    ms = torch.randn(50000, 3, 3, generator=torch.Generator().manual_seed(1)).to(cuda_dev)
+    ms, gr = [t[:MINV_REF_N].to(cuda_dev) for t in _minv_inputs()]
     a, ac = FastMinv.Fast3x3Minv(ms)
-    b, bc = ref.Fast3x3Minv(ms)
-    torch.cuda.synchronize()
+    b, bc = torch.from_numpy(ref["minv_inv"]).to(cuda_dev), torch.from_numpy(ref["minv_mask"]).to(cuda_dev)
     assert torch.equal(ac, bc), "singularity mask identical to the reference kernel"
     det = torch.linalg.det(ms.double()).abs().view(-1, 1, 1)
     # floating point: the 2x2 minors cancel, and FMA contraction differs between the two builds, so
@@ -94,10 +91,8 @@ def test_minv3x3_matches_reference_kernel(cuda_dev):
     ea = rel_err((a.double() * det * sgn).cpu().numpy()[m], adj[m])
     eb = rel_err((b.double() * det * sgn).cpu().numpy()[m], adj[m])
     assert ea < 5e-4 and eb < 5e-4 and ea < 2 * eb + 1e-6
-    gr = torch.randn_like(ms)
     # same inputs to both backward kernels (the inverses above differ in the last bits)
-    assert rel_err(FastMinv.Fast3x3Minv_backward(gr, a).cpu().numpy(),
-                   ref.Fast3x3Minv_backward(gr, a).cpu().numpy()) < 1e-6
+    assert rel_err(FastMinv.Fast3x3Minv_backward(gr, b).cpu().numpy(), ref["minv_bwd"]) < 1e-6
 
 
 # ------------------------------------------------------------------------------------------------
@@ -163,21 +158,20 @@ def _canon(v, f):
     return v[order], f2
 
 
+MC_REF_CASES = ((33, True), (65, False))
+MC_REF_ARGS = (0.0078125, 0.0078125, 0.0078125, -1.0, -1.0, -1.0, 0.0)
+
+
 def test_mc_matches_reference_kernel(cuda_dev):
-    ref = _ref("MCGpu")
-    if ref is None:
-        pytest.skip("oracle/_ref/MCGpu.so not built")
+    ref = golden("ref_kernels.npz")
     dropin()
     import MCGpu
-    for n, aniso in ((33, True), (129, False)):
+    for n, aniso in MC_REF_CASES:
         grid = _test_grid(n, 100 + n, aniso).to(cuda_dev)
-        args = (0.0078125, 0.0078125, 0.0078125, -1.0, -1.0, -1.0, 0.0)
-        v, f = MCGpu.mc_gpu(grid, *args)
-        rv, rf = ref.mc_gpu(grid, *args)
-        torch.cuda.synchronize()
-        assert v.shape == rv.shape and f.shape == rf.shape
+        v, f = MCGpu.mc_gpu(grid, *MC_REF_ARGS)
+        rcv, rcf = ref["mc%d_verts" % n], ref["mc%d_faces" % n]
+        assert v.shape == rcv.shape and f.shape == rcf.shape
         cv, cf = _canon(v.cpu().numpy(), f.cpu().numpy())
-        rcv, rcf = _canon(rv.cpu().numpy(), rf.cpu().numpy())
         assert np.array_equal(cv, rcv), "vertex positions bit-identical to the reference kernel"
         assert np.array_equal(cf, rcf), "faces identical after canonicalising the race-ordered ids"
 
@@ -222,15 +216,17 @@ def test_interp2x3d(cuda_dev):
         y = torch.randn(out.shape, generator=g).to(cuda_dev)
         gin = op.backward(y)
         assert abs((out * y).sum().item() - (x.to(cuda_dev) * gin).sum().item()) < 1e-3 * max(1.0, out.numel() ** 0.5)
-    r = _ref("interp2x_boundary3d")
-    if r is not None:
-        x = torch.randn(1, 1, 33, 41, 17, generator=g).to(cuda_dev)
-        a, ab = op.forward(x, 0.0)
-        b, bb = r.forward(x, 0.0)
-        torch.cuda.synchronize()
-        assert torch.equal(a, b) and torch.equal(ab, bb)
-        y = torch.randn_like(a)
-        assert torch.allclose(op.backward(y), r.backward(y), atol=1e-6)
+    # against the reference kernel (tests/golden/ref_kernels.npz)
+    ref = golden("ref_kernels.npz")
+    x, y = [t.to(cuda_dev) for t in _interp_inputs()]
+    a, ab = op.forward(x, 0.0)
+    assert np.array_equal(a.cpu().numpy(), ref["interp_out"]) and np.array_equal(ab.cpu().numpy(), ref["interp_bnd"])
+    assert np.allclose(op.backward(y).cpu().numpy(), ref["interp_bwd"], atol=1e-6)
+
+
+def _interp_inputs():
+    g = torch.Generator().manual_seed(12)
+    return torch.randn(1, 1, 17, 21, 9, generator=g), torch.randn(1, 1, 33, 41, 17, generator=g)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -267,25 +263,28 @@ def test_grid_sampler_gradcheck_first_and_second_order(cuda_dev):
     assert torch.autograd.gradcheck(GridSamplerMine3dBackwardFunction.apply, (inp, grid, go))
 
 
+def _grid_sampler_inputs():
+    g = torch.Generator().manual_seed(5)
+    inp = torch.rand(1, 24, 9, 17, 11, generator=g)
+    grid = (torch.rand(1, 1, 1, 1000, 3, generator=g) - 0.5) * 2.2
+    go = torch.randn(1, 24, 1, 1, 1000, generator=g)
+    return inp, grid, go, torch.randn(inp.shape, generator=g), torch.randn(grid.shape, generator=g)
+
+
 def test_grid_sampler_matches_reference_kernels(cuda_dev):
-    r = _ref("GridSamplerMine")
-    if r is None:
-        pytest.skip("oracle/_ref/GridSamplerMine.so not built")
+    ref = golden("ref_kernels.npz")
     dropin()
     import GridSamplerMine as op
-    g = torch.Generator().manual_seed(5)
-    inp = torch.rand(1, 24, 9, 17, 11, generator=g).to(cuda_dev)
-    grid = ((torch.rand(1, 1, 1, 3000, 3, generator=g) - 0.5) * 2.2).to(cuda_dev)
-    a, b = op.forward(inp, grid, 0, 1), r.forward(inp, grid, 0, 1)
-    assert torch.equal(a, b), "forward bit-identical to the reference kernel"
-    go = torch.randn_like(a)
-    (gi, gg), (ri, rg) = op.backward(inp, grid, go, 0, 1), r.backward(inp, grid, go, 0, 1)
-    assert torch.allclose(gi, ri, atol=1e-5) and torch.allclose(gg, rg, atol=2e-4, rtol=1e-4)
-    ggi, ggg = torch.randn_like(inp), torch.randn_like(grid)
+    inp, grid, go, ggi, ggg = [t.to(cuda_dev) for t in _grid_sampler_inputs()]
+    a = op.forward(inp, grid, 0, 1)
+    assert np.array_equal(a.cpu().numpy(), ref["gs_fwd"]), "forward bit-identical to the reference kernel"
+    gi, gg = op.backward(inp, grid, go, 0, 1)
+    ri, rg = torch.from_numpy(ref["gs_bwd_input"]), torch.from_numpy(ref["gs_bwd_grid"])
+    assert torch.allclose(gi.cpu(), ri, atol=1e-5) and torch.allclose(gg.cpu(), rg, atol=2e-4, rtol=1e-4)
     o = op.dbackward(ggi, ggg, inp, grid, go, 0, 1)
-    ro = r.dbackward(ggi, ggg, inp, grid, go, 0, 1)
-    for x, y in zip(o, ro):
-        assert rel_err(x.cpu().numpy(), y.cpu().numpy()) < 1e-4
+    assert len(o) == len([k for k in ref.files if k.startswith("gs_dbwd")])
+    for i, x in enumerate(o):
+        assert rel_err(x.cpu().numpy(), ref["gs_dbwd%d" % i]) < 1e-4
 
 
 # ------------------------------------------------------------------------------------------------
@@ -531,27 +530,6 @@ def test_seg3d_gather_scatter_match_the_torch_sequence(cuda_dev):
     assert torch.equal(grid, before)
 
 
-def test_tc_pair_kernel_matches_single_cta_kernel(cuda_dev, monkeypatch):
-    """cta_group::2 kernel vs the single-CTA kernel: same operands, same MMA terms and order."""
-    import subprocess, sys, os, json
-    code = (
-        "import torch, json, sys; sys.path.insert(0, %r); from selfreconcode_b200 import ops; "
-        "from selfreconcode_b200._lib import SR_ACT_SOFTPLUS100; torch.manual_seed(0); "
-        "M=777; x=torch.randn(M,512,device='cuda'); w=torch.randn(512,512,device='cuda')/22.6; "
-        "b=torch.randn(512,device='cuda')*0.01; A=ops.tc_pack_rows(x); W=ops.tc_pack_weights(w); "
-        "o=ops.tc_linear(A,W,b,M,512,512,512,SR_ACT_SOFTPLUS100,want_out=True)[1]; "
-        "print(json.dumps(dict(s=float(o.double().sum()), a=float(o.double().abs().sum()), m=float(o.max()))))"
-    ) % helpers_root()
-    outs = []
-    for pair in ("1", "0"):
-        env = dict(os.environ, SELFRECON_B200_TC_PAIR=pair)
-        r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, env=env, timeout=240)
-        assert r.returncode == 0, r.stderr[-2000:]
-        outs.append(json.loads(r.stdout.strip().splitlines()[-1]))
-    for k in outs[0]:
-        assert abs(outs[0][k] - outs[1][k]) <= 1e-6 * abs(outs[1][k]), outs
-
-
 def test_seg3d_lossless_vs_golden_and_mc(cuda_dev):
     dropin()
     from MCAcc import Seg3dLossless
@@ -587,7 +565,7 @@ def test_seg3d_lossless_vs_golden_and_mc(cuda_dev):
 
 
 # ------------------------------------------------------------------------------------------------
-# Tensor-core engine (tcgen05, split-BF16 operands, fp32 accumulation in TMEM)
+# Tensor-core engine (wgmma, split-BF16 operands, fp32 accumulation)
 # ------------------------------------------------------------------------------------------------
 def test_tc_linear_split_bf16_matches_fp64(cuda_dev):
     from selfreconcode_b200 import ops

@@ -1,7 +1,7 @@
 """GPU: the training half of the tensor-core engine (selfreconcode_b200/train_ops.py) against plain torch
 fp64 autograd of the same computation.
 
-  * sr_tc_wgrad (MN-major tcgen05 GEMM over the tiled activations) vs delta^T x
+  * sr_tc_wgrad (MN-major wgmma GEMM over the tiled activations) vs delta^T x
   * TcMlpFunction forward / backward with 1 row per point (first order) and 4 rows per point (value + 3 forward
     tangents: the backward contains act'' -- what the reference gets from double backward), incl. the SDF's skip
     connection and narrow first / last layers."""

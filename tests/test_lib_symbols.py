@@ -33,7 +33,7 @@ def test_binding_table_matches_header():
     assert sorted(_lib.SIGNATURES) == declared_symbols()
     lib = _lib.load()
     assert lib.sr_abi_version() == 1
-    assert b"sm_100a" in lib.sr_build_info()
+    assert b"sm_90a" in lib.sr_build_info()
 
 
 def test_struct_layouts_match_c():

@@ -157,7 +157,7 @@ def _one_step(net, data, rays, fids, fused, conf):
 
 def test_training_step_fused_vs_autograd():
     """The same optimisation step twice on the same GPU: training evaluations through the tensor-core training
-    engine (forward tangents + one reverse sweep, tcgen05 weight-gradient GEMMs) vs the torch-autograd twin
+    engine (forward tangents + one reverse sweep, wgmma weight-gradient GEMMs) vs the torch-autograd twin
     (create_graph=True double backward on cuBLAS): loss terms, dL/dTmpPs and every parameter gradient agree."""
     from selfreconcode_b200 import synth, train_ops
     net, data, rays, fids = build()

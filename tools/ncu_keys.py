@@ -1,4 +1,4 @@
-"""Prints the handful of ncu raw-page metrics used in profiles/*.md from a .ncu-rep."""
+"""Prints a handful of ncu raw-page metrics (DRAM bytes, tensor-pipe and issue activity) from a .ncu-rep."""
 import csv, subprocess, sys
 rep = sys.argv[1]
 raw = subprocess.run(["ncu", "-i", rep, "--page", "raw", "--csv"], capture_output=True, text=True).stdout

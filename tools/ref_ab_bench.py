@@ -1,4 +1,4 @@
-"""A/B timing on the same B200: the reference's own CUDA extensions (built from /root/reference sources
+"""A/B timing on the same GPU: the reference's own CUDA extensions (built from /root/reference sources
 into oracle/_ref/ by oracle/build.py) vs this library's kernels for the same calls ("kernel to beat",
 SURVEY.md 8d).  Measurement tooling, not product code: like tests/ it loads the checker artefacts under oracle/_ref/;
 nothing in selfreconcode_b200/ depends on it.  CUDA events, median of 10 after 3 warm-ups, whole call as the reference's user makes it."""

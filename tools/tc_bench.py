@@ -1,4 +1,4 @@
-"""Throughput of one tcgen05 split-BF16 layer (512x512) vs the FFMA engine's per-layer rate."""
+"""Throughput of one wgmma split-BF16 layer (512x512) vs the FFMA engine's per-layer rate."""
 import json, os, sys
 import numpy as np, torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))

@@ -1,5 +1,6 @@
-"""Accuracy / speed of the BF16 split GEMM with 6, 4 or 3 product terms (variant builds with
--DSR_TC_TERMS=k; run on the GPU box with SELFRECON_B200_LIB pointing at each)."""
+"""Accuracy / speed of the split-BF16 layer GEMM against fp32 / fp64 references.  Compare the 2-plane (3 terms,
+default) and 3-plane (6 terms) builds: build.build_variant("p3", ["SR_TC_PLANES=3"]), then run this script once per
+library with SELFRECON_B200_LIB pointing at it."""
 import json, os, sys
 import numpy as np, torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
