@@ -301,31 +301,6 @@ int sr_tc_linear(const void* A, const void* W, const float* bias, int64_t M, int
                  int out_col0, int out_n, float* dstash, const void* mul_tiles, int mul_K, int mul_act,
                  float mul_scale, const int32_t* m_dev, cudaStream_t s);
 
-/* One step of a whole-sweep launch: the arguments of sr_tc_linear for one layer (pointers first, then ints). */
-typedef struct sr_tc_step {
-  const void* A;          /* tiled input activations (width K) */
-  const void* W;          /* packed weights (sr_tc_pack_weights) */
-  const float* bias;      /* [pad256(N)] */
-  void* A_next;           /* tiled output (width K_next) or NULL */
-  const float* skip_src;  /* fp32 rows appended after column n_valid (skip connection) or NULL */
-  float* out;             /* fp32 row-major output or NULL */
-  const void* mul_tiles;  /* reverse step: the forward sweep's activation tiles of the previous layer, or NULL */
-  float* dstash;          /* fp32 act'(z) stash (training) or NULL */
-  int32_t N, K, n_valid, act, K_next, skip_n, skip_ld, out_ld, out_col0, out_n, mul_K, mul_act;
-  float scale, mul_scale;
-} sr_tc_step;
-
-/* sr_tc_sweep: L <= 12 chained steps (step l+1 reads the tiles step l wrote) in ONE launch: a CTA keeps its
- * row tiles through all steps, the only inter-step dependency is inside a CTA (network.py:66-83 ImplicitNetwork.forward
- * layer loop; its reverse for the tracer's gradient, FindSurfacePs.py:128-140).  Same results as L sr_tc_linear calls.
- * Restrictions: activations NONE / SOFTPLUS100 / RELU; a buffer must not be used with two different tile widths
- * (SR_EINVAL).  m_dev: optional device-side row count. */
-int sr_tc_sweep(const sr_tc_step* steps, int L, int64_t M, int ch, const int32_t* m_dev, cudaStream_t s);
-/* tuning knock-outs of the whole-sweep kernel (measurement only; bit 0 drops the epilogue's proxy fence and makes the
- * results undefined).  Returns the previous flags. */
-int sr_tc_debug_sweep_flags(int flags);
-
-
 /* Mesh rasteriser for the ray seed (replaces pytorch3d.renderer.MeshRasterizer in model/network.py:492 / :345 with
  * faces_per_pixel = 1, blur_radius = 0, perspective_correct = True; consumer: utils/FindSurfacePs.py:5-29).
  * verts_screen [N,V,3] = (pixel x = column, pixel y = row, camera depth z); faces [F,3] int64; keys = scratch of
@@ -353,9 +328,11 @@ int sr_tc_colsum(const void* T, int64_t M, int K, int ch, float* partial, int sl
 int sr_tc_unpack_rows(const void* T, int64_t M, int K, int Kpad, float* out, int ld, cudaStream_t s);
 
 /* Whole-sweep entry points: all launches of one forward / backward evaluation of an MLP from ONE call (per-layer
- * operands = the module's persistent packs).  forward: x0 [M, ld] fp32 rows -> out [M, n_last]; keeps the input tiles
- * (A_in), every hidden layer's activation tiles (acts[i], sr_tc_act_bytes(M, k_{i+1})) and, for softplus layers, the fp32
- * act'(z) (stashes[i] [M, pad256(n_i)] or NULL).  backward: gout [M, n_last] -> dW[l] [n,k] / db[l] [n] (NULL entries are
+ * operands = the module's persistent packs).  forward: x0 [M, ld] fp32 rows (ld a multiple of 32, the first d_in
+ * columns = the embedded input) -> out [M, n_out] (n_out = 0: all n_last columns); a skip layer's input is
+ * cat(previous output, x0[:, :d_in]) / sqrt(2).  Keeps the input tiles (A_in), every hidden layer's activation tiles
+ * (acts[i], sr_tc_act_bytes(M, k_{i+1})) and, for softplus layers, the fp32 act'(z) (stashes[i] [M, pad256(n_i)] or
+ * NULL).  m_dev (may be NULL): device-side row count <= M (active rays).  backward: gout [M, n_last] -> dW[l] [n,k] / db[l] [n] (NULL entries are
  * skipped) and x0_grad [M, ld] (or NULL); D0 / D1 = two delta tile buffers of sr_tc_act_bytes(M, widest layer),
  * part = sr_tc_wgrad_partial_bytes scratch for the widest pair, colsum_ws = colsum_slices x widest floats,
  * g_skip [M, g_skip_ld] scratch when a layer has a skip connection. */
@@ -367,7 +344,8 @@ typedef struct sr_tc_layer {
   int n, k, act, skip;
 } sr_tc_layer;
 int sr_tc_mlp_forward(const sr_tc_layer* layers, int L, const float* x0, int64_t M, int ld, int d_in, int ch, void* A_in,
-                      void* const* acts, float* const* stashes, float* out, cudaStream_t s);
+                      void* const* acts, float* const* stashes, float* out, const int32_t* m_dev, int n_out,
+                      cudaStream_t s);
 int sr_tc_mlp_backward(const sr_tc_layer* layers, int L, int64_t M, int ld, int d_in, int ch, const float* gout,
                        const void* A_in, void* const* acts, float* const* stashes, void* D0, void* D1, float* part,
                        float* colsum_ws, int colsum_slices, float* const* dW, float* const* db, float* x0_grad,
@@ -415,7 +393,7 @@ int sr_sdf_forward_small(const sr_mlp_desc* net, const float* pts, int64_t P, co
                          const int32_t* m_dev, float* sdf, void* work, int cap, cudaStream_t s);
 
 /* Pointwise stages of the tensor-core tracer (one OptimizeSurfacePs iteration =
- * embed -> sr_tc_linear x layers (forward, activations kept per layer) -> sr_tc_trace_mid -> sr_tc_linear x
+ * embed -> sr_tc_mlp_forward (activations kept per layer) -> sr_tc_trace_mid -> sr_tc_linear x
  * layers (reverse sweep, mul_tiles = the forward activations) -> sr_tc_trace_update).  All take an optional active
  * list + device-side count so the host never synchronises.  pw_s / pw_d are HOST arrays. */
 int sr_tc_trace_mid(const int32_t* index, const int32_t* m_dev, int64_t P, const float* pts,

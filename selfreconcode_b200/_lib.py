@@ -45,16 +45,6 @@ class TcLayer(C.Structure):
                 ("n", C.c_int), ("k", C.c_int), ("act", C.c_int), ("skip", C.c_int)]
 
 
-class TcStep(C.Structure):
-    """struct sr_tc_step: one step of sr_tc_sweep (the arguments of sr_tc_linear for one layer)."""
-    _fields_ = [("A", C.c_void_p), ("W", C.c_void_p), ("bias", C.c_void_p), ("A_next", C.c_void_p),
-                ("skip_src", C.c_void_p), ("out", C.c_void_p), ("mul_tiles", C.c_void_p), ("dstash", C.c_void_p),
-                ("N", C.c_int32), ("K", C.c_int32), ("n_valid", C.c_int32), ("act", C.c_int32),
-                ("K_next", C.c_int32), ("skip_n", C.c_int32), ("skip_ld", C.c_int32), ("out_ld", C.c_int32),
-                ("out_col0", C.c_int32), ("out_n", C.c_int32), ("mul_K", C.c_int32), ("mul_act", C.c_int32),
-                ("scale", C.c_float), ("mul_scale", C.c_float)]
-
-
 class WnLayer(C.Structure):
     """struct sr_wn_layer (weight-norm forward / backward over several layers)."""
     _fields_ = [("v", C.c_void_p), ("g", C.c_void_p), ("w", C.c_void_p), ("inv_norm", C.c_void_p),
@@ -122,8 +112,6 @@ SIGNATURES = {
     "sr_tc_pack_weights": (C.c_int, [c_f, i32, i32, i32, c_f, stream_t]),
     "sr_tc_linear": (C.c_int, [c_f, c_f, c_f, i64, i32, i32, i32, i32, i32, c_f, i32, f32, c_f, i32,
                                i32, c_f, i32, i32, i32, c_f, c_f, i32, i32, f32, c_f, stream_t]),
-    "sr_tc_sweep": (C.c_int, [C.POINTER(TcStep), i32, i64, i32, c_f, stream_t]),
-    "sr_tc_debug_sweep_flags": (C.c_int, [i32]),
     "sr_tc_trace_mid": (C.c_int, [c_f, c_f, i64, c_f, c_f, c_f, c_f, c_f, C.POINTER(LbsParams),
                                   C.POINTER(TraceParams), i32, c_f, c_f, c_f, i32, c_f, c_f, c_f, f32, f32,
                                   stream_t]),
@@ -133,7 +121,7 @@ SIGNATURES = {
     "sr_tc_wgrad_partial_bytes": (i64, [i64, i32, i32, C.POINTER(C.c_int)]),
     "sr_tc_debug_wgrad_desc_swap": (None, [i32]),
     "sr_tc_mlp_forward": (C.c_int, [C.POINTER(TcLayer), i32, c_f, i64, i32, i32, i32, c_f, C.POINTER(C.c_void_p),
-                                    C.POINTER(C.c_void_p), c_f, stream_t]),
+                                    C.POINTER(C.c_void_p), c_f, c_f, i32, stream_t]),
     "sr_tc_mlp_backward": (C.c_int, [C.POINTER(TcLayer), i32, i64, i32, i32, i32, c_f, c_f, C.POINTER(C.c_void_p),
                                      C.POINTER(C.c_void_p), c_f, c_f, c_f, c_f, i32, C.POINTER(C.c_void_p),
                                      C.POINTER(C.c_void_p), c_f, c_f, i32, stream_t]),

@@ -8,7 +8,7 @@
 // dominated by the NUMBER of accumulations (K/16 per term) rather than by the dropped terms (tools/tc_terms.py
 // compares the two builds).
 //
-// One launch runs one layer  C[M x N] = act(A[M x K] * W^T + b)  over all row tiles, or a whole sweep of layers:
+// One launch runs one layer  C[M x N] = act(A[M x K] * W^T + b)  over all row tiles:
 //   * operands live in global memory already in the canonical (no-swizzle, K-major) shared memory layout
 //     of the wgmma descriptors -- 128-byte core matrices (8 rows x 8 bf16), tiles of 128 (or 256) rows
 //     x 32 k, the split planes of a tile contiguous -- so ONE TMA bulk copy (cp.async.bulk + mbarrier)
@@ -316,25 +316,17 @@ __device__ __forceinline__ void epi_chunk(const LayerArgs& a, const EpiRow& r, u
 }
 
 
-// ---- the layer kernel: all layers of a forward or reverse sweep in ONE launch ----------------------------------
-// A CTA keeps its row tiles through every layer of the sweep: CTA c owns the row tiles {c, c + grid, ...} in EVERY
-// step.  The activations a step's epilogue writes for rows R are exactly what the same CTA loads as the next step's A
-// operand for rows R, so the only dependency between steps is inside a CTA: the producer waits until the eight
-// epilogue warps have finished the previous step on that row tile (per-warp progress counters in shared memory,
-// release / acquire, with a generic->async proxy fence on both sides because the tiles are written with st.global and
-// read back by the bulk-copy engine).  No grid barrier between layers, one barrier set-up and one launch ramp per
-// SWEEP instead of per layer; the smem ring keeps rolling across the layer boundary, so the loads of step l+1 overlap
-// the last epilogue of step l.  A single layer (sr_tc_linear) is a sweep of one step.
-// Narrow steps (N < 256: the SDF's last layer, the input gradient of the reverse sweep) run as one N = 256 tile on
-// zero-padded weight rows.  Buffers that hold tiles of different widths must be distinct: tile (mt, kc) sits at
-// (mt * KC + kc), so two layouts of one buffer alias ACROSS row tiles (the host wrapper checks this).
+// ---- the layer kernel: one layer per launch ------------------------------------------------------------------------
+// The name tc_sweep_kernel is kept: the benchmark's roofline label names it and tools/prof_train_kernels.py matches it.
+// Persistent CTAs, at most one per SM: CTA c owns the row tiles {c, c + grid, ...} and runs every n-tile of each.
+// Narrow layers (N < 256: the SDF's last layer, the input gradient of the reverse sweep) run as one N = 256 tile on
+// zero-padded weight rows.
 //
 // Roles (3 warpgroups): warpgroup 0 = TMA producer (one thread), warpgroups 1 and 2 = rows [0, 64) and [64, 128) of
 // the 128 x 256 output tile: wgmma m64n256k16 with fp32 accumulators in registers (128 per thread), then the
 // epilogue of the same rows.  The accumulator goes through shared memory (128 columns at a time) so that each
 // epilogue thread owns one row and 32 consecutive columns per chunk: the four rows of a point (value + 3 tangents)
 // sit in four consecutive lanes.
-constexpr int kMaxSteps = 12;
 constexpr int kConsumerWGs = 2;
 constexpr int kThreads = 128 * (1 + kConsumerWGs);
 constexpr int kEpiWarps = 4 * kConsumerWGs;
@@ -342,28 +334,6 @@ constexpr int STG_LD = 132;                 // staging row pitch (floats): confl
 constexpr int STG_FLOATS = 64 * STG_LD;     // per consumer warpgroup: 64 rows x 128 columns
 constexpr size_t kSmem = (size_t)STAGES * (A_STAGE_BYTES + W_STAGE_BYTES) + (size_t)kConsumerWGs * STG_FLOATS * 4 + 256;
 static_assert(kSmem <= 227 * 1024, "shared memory of one H100 block");
-struct StepArgs {
-  LayerArgs la;
-  int act;       // SR_ACT_* of a forward step / of the PREVIOUS layer for a reverse (mul) step
-  int mul;       // 1: reverse step (acc * act'(z_prev))
-};
-struct SweepArgs {
-  StepArgs step[kMaxSteps];
-  int L;
-  int dbg;          // tuning knock-outs (sr_tc_debug_sweep_flags): 1 = no proxy fence in the epilogue (WRONG results)
-  int last_plain;   // the last step is a plain linear step (no activation, no act' multiply): the network's output layer
-                    // in a forward sweep, the input gradient in a reverse sweep
-};
-
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async;" ::: "memory"); }
-__device__ __forceinline__ void st_release_smem(uint32_t* p, uint32_t v) {
-  asm volatile("st.release.cta.shared::cta.u32 [%0], %1;" ::"r"(sr_smem_u32(p)), "r"(v) : "memory");
-}
-__device__ __forceinline__ uint32_t ld_acquire_smem(const uint32_t* p) {
-  uint32_t v;
-  asm volatile("ld.acquire.cta.shared::cta.u32 %0, [%1];" : "=r"(v) : "r"(sr_smem_u32(p)) : "memory");
-  return v;
-}
 
 // One k chunk of this warpgroup's 64 x 256 tile: the split-bf16 product terms, plane pairs smallest contributions
 // first -- 2 planes: (a0,w1) (a1,w0) (a0,w0); 3 planes: (a0,w2) (a2,w0) (a1,w1) (a0,w1) (a1,w0) (a0,w0).
@@ -387,9 +357,9 @@ __device__ __forceinline__ void mma_chunk(float (&acc)[128], uint32_t abase, uin
   }
 }
 
-// <ACT, MUL>: activation / mode of every step but (optionally) the last -- the two epilogues a sweep needs
+// <ACT, CH, MUL>: the layer's activation (a reverse launch: the PREVIOUS layer's), rows per point, reverse mode
 template <int ACT, int CH, bool MUL>
-__global__ void __launch_bounds__(kThreads, 1) tc_sweep_kernel(const __grid_constant__ SweepArgs sw) {
+__global__ void __launch_bounds__(kThreads, 1) tc_sweep_kernel(const __grid_constant__ LayerArgs a) {
   extern __shared__ __align__(1024) unsigned char smem[];
   __nv_bfloat16* sA = reinterpret_cast<__nv_bfloat16*>(smem);
   __nv_bfloat16* sW = reinterpret_cast<__nv_bfloat16*>(smem + (size_t)STAGES * A_STAGE_BYTES);
@@ -397,26 +367,22 @@ __global__ void __launch_bounds__(kThreads, 1) tc_sweep_kernel(const __grid_cons
   uint64_t* bars = reinterpret_cast<uint64_t*>(stg + kConsumerWGs * STG_FLOATS);
   uint64_t* full = bars;                    // [STAGES] operands of the stage landed (producer expect_tx)
   uint64_t* empty = bars + STAGES;          // [STAGES] the MMAs of every consumer warp have read the stage
-  uint32_t* done = reinterpret_cast<uint32_t*>(empty + STAGES);   // [kEpiWarps] items finished by each epilogue warp
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7;
   if (threadIdx.x == 0) {
     for (int i = 0; i < STAGES; ++i) { sr_mbar_init(&full[i], 1); sr_mbar_init(&empty[i], kEpiWarps); }
-    for (int i = 0; i < kEpiWarps; ++i) done[i] = 0u;
     sr_fence_barrier_init();
   }
   __syncthreads();
-  const LayerArgs& a0 = sw.step[0].la;
-  long long Mrows = a0.M;
-  int MTe = a0.MT;
-  if (a0.m_dev != nullptr) {
-    const long long md = (long long)(*a0.m_dev);
-    Mrows = md < a0.M ? md : a0.M;
+  long long Mrows = a.M;
+  int MTe = a.MT;
+  if (a.m_dev != nullptr) {
+    const long long md = (long long)(*a.m_dev);
+    Mrows = md < a.M ? md : a.M;
     MTe = (int)((Mrows + BM - 1) / BM);
   }
   const int cta = blockIdx.x, ncta = gridDim.x;
   const int J = cta < MTe ? (MTe - cta + ncta - 1) / ncta : 0;   // row tiles of this CTA
-  const int L = sw.L;
 
   // 384 threads at one block per SM start with 168 registers each; the producer warpgroup hands most of its share to
   // the consumers (128 accumulators + epilogue state per thread): 128 x 40 + 256 x 232 <= 65 536
@@ -426,30 +392,17 @@ __global__ void __launch_bounds__(kThreads, 1) tc_sweep_kernel(const __grid_cons
     if (threadIdx.x == 0) {
       int slot = 0;
       uint32_t phase = 0;
-      uint32_t items_before = 0;            // items of the steps before the previous one
-      for (int l = 0; l < L; ++l) {
-        const LayerArgs& a = sw.step[l].la;
-        const int NTp = l > 0 ? sw.step[l - 1].la.NT : 0;
-        for (int j = 0; j < J; ++j) {
-          const long long mt = (long long)cta + (long long)j * ncta;
-          for (int nt = 0; nt < a.NT; ++nt) {
-            for (int kc = 0; kc < a.KC; ++kc) {
-              sr_mbar_wait(&empty[slot], phase ^ 1u);
-              sr_mbar_arrive_expect_tx(&full[slot], A_STAGE_BYTES + W_STAGE_BYTES);
-              sr_bulk_g2s(sW + (size_t)slot * W_STAGE, a.W + w_tile_off(nt, kc, a.KC, 0), W_STAGE_BYTES, &full[slot]);
-              if (l > 0 && nt == 0 && kc == 0) {
-                // rows of tile j: every n-tile of the previous step must have left the epilogue
-                const uint32_t need = items_before + (uint32_t)(j + 1) * (uint32_t)NTp;
-                for (int w = 0; w < kEpiWarps; ++w)
-                  while (ld_acquire_smem(&done[w]) < need) {}
-                fence_proxy_async();
-              }
-              sr_bulk_g2s(sA + (size_t)slot * A_STAGE, a.A + a_tile_off(mt, kc, a.KC, 0), A_STAGE_BYTES, &full[slot]);
-              if (++slot == STAGES) { slot = 0; phase ^= 1u; }
-            }
+      for (int j = 0; j < J; ++j) {
+        const long long mt = (long long)cta + (long long)j * ncta;
+        for (int nt = 0; nt < a.NT; ++nt) {
+          for (int kc = 0; kc < a.KC; ++kc) {
+            sr_mbar_wait(&empty[slot], phase ^ 1u);
+            sr_mbar_arrive_expect_tx(&full[slot], A_STAGE_BYTES + W_STAGE_BYTES);
+            sr_bulk_g2s(sW + (size_t)slot * W_STAGE, a.W + w_tile_off(nt, kc, a.KC, 0), W_STAGE_BYTES, &full[slot]);
+            sr_bulk_g2s(sA + (size_t)slot * A_STAGE, a.A + a_tile_off(mt, kc, a.KC, 0), A_STAGE_BYTES, &full[slot]);
+            if (++slot == STAGES) { slot = 0; phase ^= 1u; }
           }
         }
-        if (l > 0) items_before += (uint32_t)J * (uint32_t)NTp;
       }
     }
   } else {
@@ -457,83 +410,68 @@ __global__ void __launch_bounds__(kThreads, 1) tc_sweep_kernel(const __grid_cons
     asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
     const int cw = wg - 1;                  // rows [64 cw, 64 cw + 64) of the row tile
     const int wq = warp & 3;                // warp in the warpgroup
-    const int ew = 4 * cw + wq;             // epilogue warp index
     float* st = stg + cw * STG_FLOATS;
     float acc[128];
     EpiRow r;
     r.row_in_tile = cw * 64 + (wq & 1) * 32 + lane;
     r.lane = lane;
     r.is_val = (CH == 1) || ((lane & 3) == 0);
+    r.ds_ld = (size_t)a.NT * BN;
     int slot = 0;
     uint32_t phase = 0;
-    uint32_t items = 0;
-    for (int l = 0; l < L; ++l) {
-      const LayerArgs& a = sw.step[l].la;
-      const bool plain = sw.last_plain && l == L - 1;
-      r.ds_ld = (size_t)a.NT * BN;
-      for (int j = 0; j < J; ++j) {
-        r.mt = (long long)cta + (long long)j * ncta;
-        r.row = r.mt * BM + r.row_in_tile;
-        r.row_ok = r.row < Mrows;
-        for (int nt = 0; nt < a.NT; ++nt) {
-          r.nt = nt;
-          // the first k chunk overwrites the accumulator (it is dead from here back to the previous epilogue)
+    for (int j = 0; j < J; ++j) {
+      r.mt = (long long)cta + (long long)j * ncta;
+      r.row = r.mt * BM + r.row_in_tile;
+      r.row_ok = r.row < Mrows;
+      for (int nt = 0; nt < a.NT; ++nt) {
+        r.nt = nt;
+        // the first k chunk overwrites the accumulator (it is dead from here back to the previous epilogue)
+        sr_mbar_wait(&full[slot], phase);
+        wgmma_fence();
+        mma_chunk<true>(acc, sr_smem_u32(sA + (size_t)slot * A_STAGE) + cw * 8 * 128,
+                        sr_smem_u32(sW + (size_t)slot * W_STAGE));
+        wgmma_commit();
+        int prev = slot;
+        if (++slot == STAGES) { slot = 0; phase ^= 1u; }
+        for (int kc = 1; kc < a.KC; ++kc) {
           sr_mbar_wait(&full[slot], phase);
           wgmma_fence();
-          mma_chunk<true>(acc, sr_smem_u32(sA + (size_t)slot * A_STAGE) + cw * 8 * 128,
-                          sr_smem_u32(sW + (size_t)slot * W_STAGE));
+          mma_chunk<false>(acc, sr_smem_u32(sA + (size_t)slot * A_STAGE) + cw * 8 * 128,
+                           sr_smem_u32(sW + (size_t)slot * W_STAGE));
           wgmma_commit();
-          int prev = slot;
-          if (++slot == STAGES) { slot = 0; phase ^= 1u; }
-          for (int kc = 1; kc < a.KC; ++kc) {
-            sr_mbar_wait(&full[slot], phase);
-            wgmma_fence();
-            mma_chunk<false>(acc, sr_smem_u32(sA + (size_t)slot * A_STAGE) + cw * 8 * 128,
-                             sr_smem_u32(sW + (size_t)slot * W_STAGE));
-            wgmma_commit();
-            wgmma_wait<1>();   // the previous stage's MMAs are complete: release it
-            if (lane == 0) sr_mbar_arrive(&empty[prev]);
-            prev = slot;
-            if (++slot == STAGES) { slot = 0; phase ^= 1u; }
-          }
-          wgmma_wait<0>();
+          wgmma_wait<1>();   // the previous stage's MMAs are complete: release it
           if (lane == 0) sr_mbar_arrive(&empty[prev]);
-          // epilogue: 128 accumulator columns per pass through the staging buffer; warp wq handles rows
-          // 32 (wq & 1) + lane and the 64 columns 64 (wq >> 1) of each pass (two 32-column chunks)
+          prev = slot;
+          if (++slot == STAGES) { slot = 0; phase ^= 1u; }
+        }
+        wgmma_wait<0>();
+        if (lane == 0) sr_mbar_arrive(&empty[prev]);
+        // epilogue: 128 accumulator columns per pass through the staging buffer; warp wq handles rows
+        // 32 (wq & 1) + lane and the 64 columns 64 (wq >> 1) of each pass (two 32-column chunks)
 #pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const int fr = 16 * wq + (lane >> 2), fc = 2 * (lane & 3);
+        for (int h = 0; h < 2; ++h) {
+          const int fr = 16 * wq + (lane >> 2), fc = 2 * (lane & 3);
 #pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              *reinterpret_cast<float2*>(st + fr * STG_LD + 8 * i + fc) =
-                  make_float2(acc[4 * (16 * h + i)], acc[4 * (16 * h + i) + 1]);
-              *reinterpret_cast<float2*>(st + (fr + 8) * STG_LD + 8 * i + fc) =
-                  make_float2(acc[4 * (16 * h + i) + 2], acc[4 * (16 * h + i) + 3]);
-            }
-            warpgroup_sync(1 + cw);
-            const float* srow = st + ((wq & 1) * 32 + lane) * STG_LD + (wq >> 1) * 64;
-            for (int i = 0; i < 2; ++i) {
-              const int chunk = 4 * h + 2 * (wq >> 1) + i;
-              uint32_t v[32];
-#pragma unroll
-              for (int j4 = 0; j4 < 8; ++j4) {
-                const float4 t = reinterpret_cast<const float4*>(srow + 32 * i)[j4];
-                v[4 * j4] = __float_as_uint(t.x); v[4 * j4 + 1] = __float_as_uint(t.y);
-                v[4 * j4 + 2] = __float_as_uint(t.z); v[4 * j4 + 3] = __float_as_uint(t.w);
-              }
-              const bool live = nt * BN + chunk * 32 < a.n_gemm;
-              if (plain) epi_chunk<SR_ACT_NONE, CH, false>(a, r, v, chunk, live);
-              else epi_chunk<ACT, CH, MUL>(a, r, v, chunk, live);
-            }
-            warpgroup_sync(1 + cw);
+          for (int i = 0; i < 16; ++i) {
+            *reinterpret_cast<float2*>(st + fr * STG_LD + 8 * i + fc) =
+                make_float2(acc[4 * (16 * h + i)], acc[4 * (16 * h + i) + 1]);
+            *reinterpret_cast<float2*>(st + (fr + 8) * STG_LD + 8 * i + fc) =
+                make_float2(acc[4 * (16 * h + i) + 2], acc[4 * (16 * h + i) + 3]);
           }
-          // this lane's tile stores -> visible to the bulk copies of the next step (nothing reads the last step's)
-          // (one fence + one progress update per ROW TILE: the next step needs all n-tiles of the row tile anyway)
-          ++items;
-          const bool publish = nt == a.NT - 1 && l + 1 < L;
-          if (publish && !(sw.dbg & 1)) fence_proxy_async();
-          __syncwarp();
-          if (publish && lane == 0) st_release_smem(&done[ew], items);
+          warpgroup_sync(1 + cw);
+          const float* srow = st + ((wq & 1) * 32 + lane) * STG_LD + (wq >> 1) * 64;
+          for (int i = 0; i < 2; ++i) {
+            const int chunk = 4 * h + 2 * (wq >> 1) + i;
+            uint32_t v[32];
+#pragma unroll
+            for (int j4 = 0; j4 < 8; ++j4) {
+              const float4 t = reinterpret_cast<const float4*>(srow + 32 * i)[j4];
+              v[4 * j4] = __float_as_uint(t.x); v[4 * j4 + 1] = __float_as_uint(t.y);
+              v[4 * j4 + 2] = __float_as_uint(t.z); v[4 * j4 + 3] = __float_as_uint(t.w);
+            }
+            epi_chunk<ACT, CH, MUL>(a, r, v, chunk, nt * BN + chunk * 32 < a.n_gemm);
+          }
+          warpgroup_sync(1 + cw);
         }
       }
     }
@@ -741,39 +679,32 @@ int sr_tc_pack_weights(const float* w, int N, int K, int ld, void* dst, cudaStre
   return sr_launch_status();
 }
 
-static int g_sweep_dbg = 0;
-int sr_tc_debug_sweep_flags(int flags) {
-  const int old = g_sweep_dbg;
-  g_sweep_dbg = flags;
-  return old;
-}
-
-static int tc_fill_step(const sr_tc_step& t, int64_t M, int ch, const int32_t* m_dev, sr_tc::StepArgs& st) {
+// picks the instantiation for (activation, mode, ch) and launches one CTA per row tile, at most one per SM
+int sr_tc_linear(const void* A, const void* W, const float* bias, int64_t M, int N, int K, int n_valid,
+                 int act, int ch, void* A_next, int K_next, float scale, const float* skip_src,
+                 int skip_n, int skip_ld, float* out, int out_ld, int out_col0, int out_n,
+                 float* dstash, const void* mul_tiles, int mul_K, int mul_act, float mul_scale,
+                 const int32_t* m_dev, cudaStream_t s) {
   using namespace sr_tc;
-  if (!t.A || !t.W || !t.bias || t.N <= 0 || t.K <= 0 || (!t.A_next && !t.out)) return SR_EINVAL;
-  if (t.mul_tiles && t.mul_K < t.n_valid) return SR_EINVAL;
-  LayerArgs& a = st.la;
-  a.A = (const __nv_bfloat16*)t.A; a.W = (const __nv_bfloat16*)t.W; a.bias = t.bias; a.M = M;
-  a.MT = (int)((M + BM - 1) / BM); a.NT = (t.N + BN - 1) / BN; a.KC = (t.K + 31) / 32;
-  a.n_gemm = t.N; a.n = t.n_valid; a.ch = ch;
-  a.A_next = (__nv_bfloat16*)t.A_next; a.KCn = t.A_next ? (t.K_next + 31) / 32 : 0;
-  a.scale = t.scale; a.skip_src = t.skip_src; a.skip_n = t.skip_n; a.skip_ld = t.skip_ld;
-  a.out = t.out; a.out_ld = t.out_ld; a.dstash = t.dstash; a.out_col0 = t.out_col0; a.out_n = t.out_n;
-  a.mul_tiles = (const __nv_bfloat16*)t.mul_tiles; a.mul_KC = (t.mul_K + 31) / 32;
-  a.mul_inv_scale = t.mul_scale != 0.f ? 1.0f / t.mul_scale : 1.0f; a.m_dev = m_dev;
-  st.mul = t.mul_tiles ? 1 : 0;
-  st.act = t.mul_tiles ? t.mul_act : t.act;
-  return SR_OK;
-}
+  if (M <= 0 || (ch != 1 && ch != 4)) return SR_EINVAL;
+  if (!A || !W || !bias || N <= 0 || K <= 0 || (!A_next && !out)) return SR_EINVAL;
+  if (mul_tiles ? (mul_K < n_valid || (mul_act != SR_ACT_NONE && mul_act != SR_ACT_SOFTPLUS100 && mul_act != SR_ACT_RELU))
+                : (act < SR_ACT_NONE || act > SR_ACT_TANH))
+    return SR_EINVAL;
+  LayerArgs a;
+  a.A = (const __nv_bfloat16*)A; a.W = (const __nv_bfloat16*)W; a.bias = bias; a.M = M;
+  a.MT = (int)((M + BM - 1) / BM); a.NT = (N + BN - 1) / BN; a.KC = (K + 31) / 32;
+  a.n_gemm = N; a.n = n_valid; a.ch = ch;
+  a.A_next = (__nv_bfloat16*)A_next; a.KCn = A_next ? (K_next + 31) / 32 : 0;
+  a.scale = scale; a.skip_src = skip_src; a.skip_n = skip_n; a.skip_ld = skip_ld;
+  a.out = out; a.out_ld = out_ld; a.dstash = dstash; a.out_col0 = out_col0; a.out_n = out_n;
+  a.mul_tiles = (const __nv_bfloat16*)mul_tiles; a.mul_KC = (mul_K + 31) / 32;
+  a.mul_inv_scale = mul_scale != 0.f ? 1.0f / mul_scale : 1.0f; a.m_dev = m_dev;
 
-// picks the instantiation for (body activation, mode, ch) and launches one CTA per row tile, at most one per SM
-static int tc_launch_sweep(sr_tc::SweepArgs& sw, int ch, cudaStream_t s) {
-  using namespace sr_tc;
-  const StepArgs& b = sw.step[0];
-  using Kern = void (*)(const SweepArgs);
+  using Kern = void (*)(const LayerArgs);
   Kern kern = nullptr;
 #define SR_SW(ACT_, CH_, MUL_) kern = (Kern)tc_sweep_kernel<ACT_, CH_, MUL_>
-  const int key = (ch == 4 ? 10 : 0) + (b.mul ? 5 : 0) + b.act;
+  const int key = (ch == 4 ? 10 : 0) + (mul_tiles ? 5 + mul_act : act);
   switch (key) {
     case 0: SR_SW(SR_ACT_NONE, 1, false); break;
     case 1: SR_SW(SR_ACT_SOFTPLUS100, 1, false); break;
@@ -802,65 +733,8 @@ static int tc_launch_sweep(sr_tc::SweepArgs& sw, int ch, cudaStream_t s) {
     if (e != cudaSuccess) return (int)e;
     attr_set = true;
   }
-  const int MT = b.la.MT;
-  const int grid = MT < SR_NUM_SMS ? MT : SR_NUM_SMS;
-  kern<<<grid, kThreads, kSmem, s>>>(sw);
+  const int grid = a.MT < SR_NUM_SMS ? a.MT : SR_NUM_SMS;
+  kern<<<grid, kThreads, kSmem, s>>>(a);
   return sr_launch_status();
-}
-
-int sr_tc_linear(const void* A, const void* W, const float* bias, int64_t M, int N, int K, int n_valid,
-                 int act, int ch, void* A_next, int K_next, float scale, const float* skip_src,
-                 int skip_n, int skip_ld, float* out, int out_ld, int out_col0, int out_n,
-                 float* dstash, const void* mul_tiles, int mul_K, int mul_act, float mul_scale,
-                 const int32_t* m_dev, cudaStream_t s) {
-  using namespace sr_tc;
-  if (M <= 0 || (ch != 1 && ch != 4)) return SR_EINVAL;
-  sr_tc_step t = {};
-  t.A = A; t.W = W; t.bias = bias; t.A_next = A_next; t.skip_src = skip_src; t.out = out;
-  t.mul_tiles = mul_tiles; t.dstash = dstash;
-  t.N = N; t.K = K; t.n_valid = n_valid; t.act = act; t.K_next = K_next; t.skip_n = skip_n; t.skip_ld = skip_ld;
-  t.out_ld = out_ld; t.out_col0 = out_col0; t.out_n = out_n; t.mul_K = mul_K; t.mul_act = mul_act;
-  t.scale = scale; t.mul_scale = mul_scale;
-  if (mul_tiles ? (mul_act != SR_ACT_NONE && mul_act != SR_ACT_SOFTPLUS100 && mul_act != SR_ACT_RELU)
-                : (act < SR_ACT_NONE || act > SR_ACT_TANH))
-    return SR_EINVAL;
-  SweepArgs sw;
-  sw.L = 1;
-  sw.dbg = 0;
-  sw.last_plain = 0;
-  const int rc = tc_fill_step(t, M, ch, m_dev, sw.step[0]);
-  if (rc) return rc;
-  return tc_launch_sweep(sw, ch, s);
-}
-
-int sr_tc_sweep(const sr_tc_step* steps, int L, int64_t M, int ch, const int32_t* m_dev, cudaStream_t s) {
-  using namespace sr_tc;
-  if (!steps || L <= 0 || L > kMaxSteps || M <= 0 || (ch != 1 && ch != 4)) return SR_EINVAL;
-  SweepArgs sw;
-  sw.L = L;
-  sw.dbg = g_sweep_dbg;
-  for (int l = 0; l < L; ++l) {
-    const sr_tc_step& t = steps[l];
-    if (t.act != SR_ACT_NONE && t.act != SR_ACT_SOFTPLUS100 && t.act != SR_ACT_RELU) return SR_EINVAL;
-    if (t.mul_tiles && (t.mul_act != SR_ACT_NONE && t.mul_act != SR_ACT_SOFTPLUS100 && t.mul_act != SR_ACT_RELU))
-      return SR_EINVAL;
-    const int rc = tc_fill_step(t, M, ch, m_dev, sw.step[l]);
-    if (rc) return rc;
-  }
-  // one buffer, two tile widths: the layouts alias across row tiles, and CTAs run through the steps unsynchronised
-  for (int i = 0; i < L; ++i)
-    for (int j = 0; j < L; ++j) {
-      const LayerArgs &x = sw.step[i].la, &y = sw.step[j].la;
-      if (x.A_next && x.A_next == y.A_next && x.KCn != y.KCn) return SR_EINVAL;
-      if (x.A_next && (const void*)x.A_next == (const void*)y.A && x.KCn != y.KC) return SR_EINVAL;
-      if (x.A == y.A && x.KC != y.KC) return SR_EINVAL;
-    }
-  // every step but an optional plain last one shares (activation, mode)
-  const int body_act = sw.step[0].act, body_mul = sw.step[0].mul;
-  const StepArgs& lastp = sw.step[L - 1];
-  sw.last_plain = !lastp.mul && lastp.act == SR_ACT_NONE && (body_mul || body_act != SR_ACT_NONE) ? 1 : 0;
-  for (int l = 0; l < L - (sw.last_plain ? 1 : 0); ++l)
-    if (sw.step[l].act != body_act || sw.step[l].mul != body_mul) return SR_EINVAL;
-  return tc_launch_sweep(sw, ch, s);
 }
 }

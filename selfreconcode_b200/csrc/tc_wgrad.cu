@@ -355,10 +355,12 @@ int sr_tc_pack_rows(const float* src, int64_t M, int K, int ld, void* dst, const
 static inline int pad_to(int x, int m) { return (x + m - 1) / m * m; }
 
 int sr_tc_mlp_forward(const sr_tc_layer* layers, int L, const float* x0, int64_t M, int ld, int d_in, int ch, void* A_in,
-                      void* const* acts, float* const* stashes, float* out, cudaStream_t s) {
-  if (!layers || L <= 0 || L > 16 || !x0 || M <= 0 || ld <= 0 || (ld % 32) != 0 || !A_in || !out || (L > 1 && !acts))
+                      void* const* acts, float* const* stashes, float* out, const int32_t* m_dev, int n_out,
+                      cudaStream_t s) {
+  if (!layers || L <= 0 || L > 16 || !x0 || M <= 0 || ld <= 0 || (ld % 32) != 0 || !A_in || !out || (L > 1 && !acts) ||
+      n_out < 0 || n_out > layers[L - 1].n)
     return SR_EINVAL;
-  int rc = sr_tc_pack_rows(x0, M, ld, ld, A_in, nullptr, s);
+  int rc = sr_tc_pack_rows(x0, M, ld, ld, A_in, m_dev, s);
   if (rc) return rc;
   const void* cur = A_in;
   int K = ld;
@@ -367,10 +369,11 @@ int sr_tc_mlp_forward(const sr_tc_layer* layers, int L, const float* x0, int64_t
     const bool last = i == L - 1;
     const bool skip_next = !last && layers[i + 1].skip;
     const int Kn = last ? 0 : pad_to(layers[i + 1].k, 32);
-    rc = sr_tc_linear(cur, ly.W, ly.bias, M, ly.n, K, ly.n, ly.act, ch, last ? nullptr : acts[i], Kn,
+    const int nv = last && n_out > 0 ? n_out : ly.n;
+    rc = sr_tc_linear(cur, ly.W, ly.bias, M, ly.n, K, nv, ly.act, ch, last ? nullptr : acts[i], Kn,
                       skip_next ? 0.70710678118654752f : 1.0f, skip_next ? x0 : nullptr, skip_next ? d_in : 0, ld,
-                      last ? out : nullptr, last ? ly.n : 0, 0, ly.n, (!last && stashes) ? stashes[i] : nullptr, nullptr, 0,
-                      0, 1.0f, nullptr, s);
+                      last ? out : nullptr, last ? nv : 0, 0, nv, (!last && stashes) ? stashes[i] : nullptr, nullptr, 0,
+                      0, 1.0f, m_dev, s);
     if (rc) return rc;
     if (!last) { cur = acts[i]; K = Kn; }
   }

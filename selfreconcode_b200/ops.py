@@ -775,23 +775,23 @@ def tc_pack_weights(w):
 
 
 def tc_linear(A, W, bias, M, N, K, n_valid, act, ch=1, K_next=0, scale=1.0, skip_src=None, skip_n=0,
-              want_out=False, want_dstash=False):
-    """One layer on the tensor-core engine.  Returns (A_next | None, out | None, dstash | None)."""
+              want_out=False):
+    """One layer on the tensor-core engine.  Returns (A_next | None, out | None, None); the last slot, where an act'
+    stash could be returned, stays None."""
     lib = _lib.load()
     dev = A.device
     A_next = torch.empty((lib.sr_tc_act_bytes(M, K_next),), dtype=torch.uint8, device=dev) if K_next else None
     out = torch.empty((M, n_valid), dtype=torch.float32, device=dev) if want_out else None
     npad = (N + 255) // 256 * 256
-    ds = torch.empty((M, npad), dtype=torch.float32, device=dev) if want_dstash else None
     b = torch.zeros((npad,), dtype=torch.float32, device=dev)
     b[:bias.numel()] = bias.reshape(-1)
     with torch.cuda.device(dev):
         check(lib.sr_tc_linear(_p(A), _p(W), _p(b), M, N, K, n_valid, int(act), int(ch), _p(A_next),
                                int(K_next), float(scale), _p(skip_src), int(skip_n),
                                skip_src.shape[1] if skip_src is not None else 0, _p(out),
-                               n_valid if want_out else 0, 0, n_valid, _p(ds), None, 0, 0, 1.0, None, _stream()),
+                               n_valid if want_out else 0, 0, n_valid, None, None, 0, 0, 1.0, None, _stream()),
               "tc_linear")
-    return A_next, out, ds
+    return A_next, out, None
 
 
 class TcNet:
@@ -814,6 +814,11 @@ class TcNet:
             self.layers.append(dict(W=W, Wb=Wb, bias=torch.zeros((_pad(n, 256),), dtype=torch.float32, device=dev),
                                     n=n, k=k, act=ly.act, skip=bool(ly.skip), _e=e,
                                     zero_bias=torch.zeros((_pad(k, 256),), dtype=torch.float32, device=dev)))
+        # the same packs as sr_tc_mlp_forward's layer array (repack() keeps the buffers, so the pointers stay valid)
+        self.c_layers = (_lib.TcLayer * len(self.layers))()
+        for c, L in zip(self.c_layers, self.layers):
+            c.W, c.Wb, c.bias, c.zero_bias = (L[t].data_ptr() for t in ("W", "Wb", "bias", "zero_bias"))
+            c.n, c.k, c.act, c.skip = L["n"], L["k"], L["act"], int(L["skip"])
         self.repack()
 
     def repack(self):
@@ -837,55 +842,24 @@ def tc_net(fused):
     return t
 
 
-TC_SWEEP = _os.environ.get("SELFRECON_B200_TC_SWEEP", "0") != "0"   # off by default: one launch per layer
-_SWEEP_ACTS = (0, 1, 2)      # SR_ACT_NONE / SOFTPLUS100 / RELU: what the whole-sweep kernel's epilogues cover
-_STEP_DEFAULTS = dict(A_next=None, K_next=0, scale=1.0, skip_src=None, skip_n=0, skip_ld=0, out=None, out_ld=0,
-                      out_col0=0, out_n=0, dstash=None, mul_tiles=None, mul_K=0, mul_act=0, mul_scale=1.0)
+def _tc_mlp(lib, tcn, x0, ch, out, A_in=None, acts=None, m_dev=None):
+    """Embedded input rows x0 fp32 [M][ld] -> the last layer's first out.shape[1] columns in `out` (one pack, then one
+    wgmma launch per layer).  A_in / acts receive the input tiles and every hidden layer's output tiles when the caller
+    keeps them (the tracer's reverse sweep recomputes act' from them); m_dev: optional device-side row count."""
+    global LAUNCHES
+    M, ld = x0.shape
+    L = len(tcn.layers)
+    if A_in is None:
+        A_in = torch.empty((lib.sr_tc_act_bytes(M, ld),), dtype=torch.uint8, device=x0.device)
+        acts = [torch.empty((lib.sr_tc_act_bytes(M, _pad(ly["k"], 32)),), dtype=torch.uint8, device=x0.device)
+                for ly in tcn.layers[1:]]
+    acts_c = (C.c_void_p * max(L - 1, 1))(*[a.data_ptr() for a in acts])
+    check(lib.sr_tc_mlp_forward(tcn.c_layers, L, _p(x0), M, ld, tcn.fused.desc.d_in, ch, _p(A_in), acts_c, None,
+                                _p(out), _p(m_dev), out.shape[1], _stream()), "tc_mlp_forward")
+    LAUNCHES += L      # check() counted one; the call is 1 + L launches
 
 
-def _tc_step(**kw):
-    """One layer launch of the tensor-core engine as a dict of sr_tc_linear's arguments (tensors, not pointers)."""
-    d = dict(_STEP_DEFAULTS)
-    d.update(kw)
-    return d
-
-
-def _run_steps(lib, steps, M, ch, m_dev):
-    """Chained layer launches (step l+1 reads the tiles step l wrote).  The longest leading run of steps that share
-    (activation, mode) -- plus a plain linear step ending it -- goes out as ONE whole-sweep launch (sr_tc_sweep: a CTA
-    pair keeps its row tiles through all layers); anything left runs one launch per layer."""
-    n = 0
-    if TC_SWEEP and len(steps) >= 2 and steps[0]["dstash"] is None:
-        kind = lambda t: (t["mul_act"] if t["mul_tiles"] is not None else t["act"], t["mul_tiles"] is not None)
-        body = kind(steps[0])
-        if body[0] in _SWEEP_ACTS:
-            while n < len(steps) and kind(steps[n]) == body and steps[n]["dstash"] is None:
-                n += 1
-            if n < len(steps) and kind(steps[n]) == (0, False) and steps[n]["dstash"] is None:
-                n += 1
-        if n < 2 or n > 12:
-            n = 0
-    if n:
-        arr = (_lib.TcStep * n)()
-        for t, c in zip(steps[:n], arr):
-            c.A, c.W, c.bias, c.A_next = _p(t["A"]), _p(t["W"]), _p(t["bias"]), _p(t["A_next"])
-            c.skip_src, c.out, c.mul_tiles, c.dstash = _p(t["skip_src"]), _p(t["out"]), _p(t["mul_tiles"]), None
-            c.N, c.K, c.n_valid, c.act, c.K_next = t["N"], t["K"], t["n_valid"], t["act"], t["K_next"]
-            c.skip_n, c.skip_ld, c.out_ld, c.out_col0, c.out_n = t["skip_n"], t["skip_ld"], t["out_ld"], \
-                t["out_col0"], t["out_n"]
-            c.mul_K, c.mul_act, c.scale, c.mul_scale = t["mul_K"], t["mul_act"], t["scale"], t["mul_scale"]
-        check(lib.sr_tc_sweep(arr, n, M, ch, _p(m_dev), _stream()), "tc_sweep")
-    for t in steps[n:]:
-        check(lib.sr_tc_linear(_p(t["A"]), _p(t["W"]), _p(t["bias"]), M, t["N"], t["K"], t["n_valid"], t["act"], ch,
-                               _p(t["A_next"]), t["K_next"], t["scale"], _p(t["skip_src"]), t["skip_n"],
-                               t["skip_ld"], _p(t["out"]), t["out_ld"], t["out_col0"], t["out_n"], _p(t["dstash"]),
-                               _p(t["mul_tiles"]), t["mul_K"], t["mul_act"], t["mul_scale"], _p(m_dev), _stream()),
-              "tc_linear")
-    return n
-
-
-def tc_mlp_forward(fused, pts, ch=1, conds=None, batch_inds=None, pts_per_frame=0, n_out=None,
-                   want_dstash=False):
+def tc_mlp_forward(fused, pts, ch=1, conds=None, batch_inds=None, pts_per_frame=0, n_out=None):
     """Whole MLP on the tensor-core engine: embed -> pack -> one wgmma launch per layer.
     Returns out fp32 [P*ch, n_out] (last-layer outputs; tangent rows hold d out / d p_t)."""
     _need_cuda(pts)
@@ -899,38 +873,15 @@ def tc_mlp_forward(fused, pts, ch=1, conds=None, batch_inds=None, pts_per_frame=
     ld = _pad(d.d_in, 32)
     lib = _lib.load()
     emb = torch.empty((M, ld), dtype=torch.float32, device=dev)
+    out = torch.empty((M, n_out or net.layers[-1]["n"]), dtype=torch.float32, device=dev)
     pw = (C.c_float * 16)(*[d.pe_w[i] for i in range(16)])
     bi = batch_inds.contiguous().to(torch.int64) if batch_inds is not None else None
     cd = conds.detach().contiguous().float() if conds is not None else None
     with torch.cuda.device(dev):
         check(lib.sr_tc_embed(_p(pts), P, d.multires, pw, ch, _p(cd), _p(bi), int(pts_per_frame), condlen,
                               _p(emb), ld, None, None, _stream()), "tc_embed")
-        A = torch.empty((lib.sr_tc_act_bytes(M, ld),), dtype=torch.uint8, device=dev)
-        check(lib.sr_tc_pack_rows(_p(emb), M, ld, ld, _p(A), None, _stream()), "tc_pack_rows")
-        K = ld
-        out = None
-        stashes = []
-        steps = []
-        L = len(net.layers)
-        for i, ly in enumerate(net.layers):
-            last = i == L - 1
-            nxt = net.layers[i + 1] if not last else None
-            nv = ly["n"] if not (last and n_out) else n_out
-            Kn = _pad(nxt["k"], 32) if nxt else 0
-            skip_next = bool(nxt and nxt["skip"])
-            A_next = torch.empty((lib.sr_tc_act_bytes(M, Kn),), dtype=torch.uint8, device=dev) if nxt else None
-            o = torch.empty((M, nv), dtype=torch.float32, device=dev) if last else None
-            ds = torch.empty((M, _pad(ly["n"], 256)), dtype=torch.float32, device=dev) \
-                if (want_dstash and not last) else None
-            steps.append(_tc_step(A=A, W=ly["W"], bias=ly["bias"], N=ly["n"], K=K, n_valid=nv, act=ly["act"],
-                                  A_next=A_next, K_next=Kn, scale=0.7071067811865476 if skip_next else 1.0,
-                                  skip_src=emb if skip_next else None, skip_n=d.d_in if skip_next else 0, skip_ld=ld,
-                                  out=o, out_ld=nv if last else 0, out_n=nv, dstash=ds))
-            if ds is not None:
-                stashes.append(ds)
-            A, K, out = A_next, Kn, o
-        _run_steps(lib, steps, M, ch, None)
-    return (out, stashes) if want_dstash else out
+        _tc_mlp(lib, net, emb, ch, out)
+    return out
 
 
 class _TcTraceBuffers:
@@ -943,12 +894,10 @@ class _TcTraceBuffers:
         u8 = lambda n: torch.empty((n,), dtype=torch.uint8, device=dev)
         self.ld_s = _pad(sdf_net.desc.d_in, 32)
         self.emb_s = f32(P, self.ld_s)
-        # reverse-sweep staging tiles: one pair per tile width (a buffer is never seen under two widths)
-        def rev_widths(net):
-            dd = net.desc
-            return {32} | {_pad(dd.layer[l - 1].n, 32) for l in range(1, dd.n_layers)}
-        ws = rev_widths(sdf_net) | (rev_widths(def_net) if def_net is not None else set())
-        self.A = {w: [u8(lib.sr_tc_act_bytes(P, w)) for _ in range(2)] for w in sorted(ws)}
+        # reverse-sweep staging tiles (ping-pong pair), as wide as the widest cotangent of either network
+        widest = max([32] + [_pad(net.desc.layer[l].n, 32) for net in (sdf_net, def_net) if net is not None
+                             for l in range(net.desc.n_layers - 1)])
+        self.A = [u8(lib.sr_tc_act_bytes(P, widest)) for _ in range(2)]
         self.f = f32(P, 1)
         self.A_in = u8(lib.sr_tc_act_bytes(P, 256))
         self.acts_s = [u8(lib.sr_tc_act_bytes(P, _pad(sdf_net.desc.layer[i + 1].k, 32)))
@@ -967,85 +916,34 @@ class _TcTraceBuffers:
             self.gd = f32(P, 64)
             # the translator's sweeps run on a second stream beside the SDF's (own staging buffers)
             self.A_in_d = u8(lib.sr_tc_act_bytes(P, 256))
-            self.A_d = {w: [u8(lib.sr_tc_act_bytes(P, w)) for _ in range(2)] for w in sorted(rev_widths(def_net))}
+            self.A_d = [u8(lib.sr_tc_act_bytes(P, widest)) for _ in range(2)]
             self.gskip_d = f32(P, 64)
 
 
-
-
-def _tc_forward_sweep(lib, net, tcn, emb, ld, A_in, acts, P, m_dev, out):
-    """embedded input (already in `emb`) -> all layers; layer i writes its output tiles to acts[i]
-    (kept for the reverse sweep, which recomputes act' from them); last layer -> `out` fp32."""
-    d = net.desc
-    check(lib.sr_tc_pack_rows(_p(emb), P, ld, ld, _p(A_in), _p(m_dev), _stream()), "tc_pack_rows")
-    K = ld
-    cur = A_in
-    L = len(tcn.layers)
-    steps = []
-    for i, ly in enumerate(tcn.layers):
-        last = i == L - 1
-        nxt = tcn.layers[i + 1] if not last else None
-        Kn = _pad(nxt["k"], 32) if nxt else 0
-        skip_next = bool(nxt and nxt["skip"])
-        steps.append(_tc_step(A=cur, W=ly["W"], bias=ly["bias"], N=ly["n"], K=K, n_valid=ly["n"], act=ly["act"],
-                              A_next=acts[i] if nxt else None, K_next=Kn,
-                              scale=0.7071067811865476 if skip_next else 1.0, skip_src=emb if skip_next else None,
-                              skip_n=d.d_in if skip_next else 0, skip_ld=ld, out=out if last else None,
-                              out_ld=out.shape[1] if last else 0, out_n=ly["n"] if last else 0))
-        if nxt:
-            cur, K = acts[i], Kn
-    _run_steps(lib, steps, P, 1, m_dev)
-
-
-def _tc_backward_sweep(lib, net, tcn, cot, A_bufs, acts, P, m_dev, g_out, g_skip, n_keep):
+def _tc_backward_sweep(lib, tcn, cot, bufs, acts, P, m_dev, g_out, g_skip, n_keep):
     """cotangent rows `cot` [P][32] of the net outputs -> d/d(embedded input) in g_out [P][ld]
-    (first n_keep columns), skip-connection part in g_skip.  acts = the forward sweep's tiles.
-    A_bufs: per tile width one pair of staging buffers ({width: [buf, buf]}; the whole-sweep kernel must not see one
-    buffer under two widths) or, legacy, a plain pair used for every width (per-layer launches only)."""
-    d = net.desc
-    L = len(tcn.layers)
-    per_width = isinstance(A_bufs, dict)
-    flip = {}
-
-    def stage(width):
-        if not per_width:
-            i = flip.get(0, 0)
-            flip[0] = 1 - i
-            return A_bufs[i]
-        i = flip.get(width, 0)
-        flip[width] = 1 - i
-        return A_bufs[width][i]
-
-    cur = stage(32)
+    (first n_keep columns), skip-connection part in g_skip.  acts = the forward sweep's tiles; bufs = a pair of
+    staging tile buffers the layers alternate between."""
+    d_in = tcn.fused.desc.d_in
+    cur, nxt = bufs
     check(lib.sr_tc_pack_rows(_p(cot), P, 32, 32, _p(cur), _p(m_dev), _stream()), "tc_pack_rows")
     K = 32
-    steps = []
-    for l in range(L - 1, -1, -1):
+    for l in range(len(tcn.layers) - 1, -1, -1):
         ly = tcn.layers[l]
-        n_prev = tcn.layers[l - 1]["n"] if l > 0 else 0
         scale = 0.7071067811865476 if ly["skip"] else 1.0
         if l > 0:
+            n_prev = tcn.layers[l - 1]["n"]
             Kn = _pad(n_prev, 32)
-            want_skip = ly["skip"]
-            nxt = stage(Kn)
-            steps.append(_tc_step(A=cur, W=ly["Wb"], bias=ly["zero_bias"], N=ly["k"], K=K, n_valid=n_prev, act=0,
-                                  A_next=nxt, K_next=Kn, scale=scale, out=g_skip if want_skip else None,
-                                  out_ld=g_skip.shape[1] if want_skip else 0, out_col0=n_prev,
-                                  out_n=d.d_in if want_skip else 0, mul_tiles=acts[l - 1], mul_K=_pad(ly["k"], 32),
-                                  mul_act=tcn.layers[l - 1]["act"], mul_scale=scale))
-            cur, K = nxt, Kn
+            gk = g_skip if ly["skip"] else None
+            check(lib.sr_tc_linear(_p(cur), _p(ly["Wb"]), _p(ly["zero_bias"]), P, ly["k"], K, n_prev, 0, 1, _p(nxt),
+                                   Kn, scale, None, 0, 0, _p(gk), gk.shape[1] if gk is not None else 0, n_prev,
+                                   d_in if gk is not None else 0, None, _p(acts[l - 1]), _pad(ly["k"], 32),
+                                   tcn.layers[l - 1]["act"], scale, _p(m_dev), _stream()), "tc_linear")
+            cur, nxt, K = nxt, cur, Kn
         else:
-            steps.append(_tc_step(A=cur, W=ly["Wb"], bias=ly["zero_bias"], N=ly["k"], K=K, n_valid=ly["k"], act=0,
-                                  scale=scale, out=g_out, out_ld=g_out.shape[1], out_col0=0, out_n=n_keep))
-    if not per_width:
-        saved = globals()["TC_SWEEP"]
-        globals()["TC_SWEEP"] = False
-        try:
-            _run_steps(lib, steps, P, 1, m_dev)
-        finally:
-            globals()["TC_SWEEP"] = saved
-    else:
-        _run_steps(lib, steps, P, 1, m_dev)
+            check(lib.sr_tc_linear(_p(cur), _p(ly["Wb"]), _p(ly["zero_bias"]), P, ly["k"], K, ly["k"], 0, 1, None, 0,
+                                   scale, None, 0, 0, _p(g_out), g_out.shape[1], 0, n_keep, None, None, 0, 0, 1.0,
+                                   _p(m_dev), _stream()), "tc_linear")
 
 
 class _TcTraceCtx:
@@ -1113,14 +1011,14 @@ def _tc_trace_body(lib, G, sdf_net, def_net, ts, td, tp, P, times, condlen, has_
             with torch.cuda.stream(side):
                 check(lib.sr_tc_embed(_p(pts), P, dd.multires, pw_d, 1, _p(conds), _p(bi), 0, condlen,
                                       _p(B.emb_d), B.ld_d, _p(idx), _p(m_dev), _stream()), "tc_embed")
-                _tc_forward_sweep(lib, def_net, td, B.emb_d, B.ld_d, B.A_in_d, B.acts_d, P, m_dev, B.off)
-        _tc_forward_sweep(lib, sdf_net, ts, B.emb_s, B.ld_s, B.A_in, B.acts_s, P, m_dev, B.f)
+                _tc_mlp(lib, td, B.emb_d, 1, B.off, B.A_in_d, B.acts_d, m_dev)
+        _tc_mlp(lib, ts, B.emb_s, 1, B.f, B.A_in, B.acts_s, m_dev)
         if dual:
             main.wait_stream(side)
         elif def_net is not None:
             check(lib.sr_tc_embed(_p(pts), P, dd.multires, pw_d, 1, _p(conds), _p(bi), 0, condlen,
                                   _p(B.emb_d), B.ld_d, _p(idx), _p(m_dev), _stream()), "tc_embed")
-            _tc_forward_sweep(lib, def_net, td, B.emb_d, B.ld_d, B.A_in, B.acts_d, P, m_dev, B.off)
+            _tc_mlp(lib, td, B.emb_d, 1, B.off, B.A_in, B.acts_d, m_dev)
         check(lib.sr_tc_trace_mid(_p(idx), _p(m_dev), P, _p(pts), _p(rays), _p(bi), _p(B.f),
                                   _p(B.off) if def_net is not None else None, lbs_ref, C.byref(tp),
                                   1 if a_out is not None else 0, _p(conv), _p(B.cot_s),
@@ -1141,14 +1039,12 @@ def _tc_trace_body(lib, G, sdf_net, def_net, ts, td, tp, P, times, condlen, has_
         if dual:
             side.wait_stream(main)
             with torch.cuda.stream(side):
-                _tc_backward_sweep(lib, def_net, td, B.cot_d, B.A_d, B.acts_d, P, m_dev, B.gd, B.gskip_d,
-                                   3 + 6 * dd.multires)
-        _tc_backward_sweep(lib, sdf_net, ts, B.cot_s, B.A, B.acts_s, P, m_dev, B.gs, B.gskip, ds.d_in)
+                _tc_backward_sweep(lib, td, B.cot_d, B.A_d, B.acts_d, P, m_dev, B.gd, B.gskip_d, 3 + 6 * dd.multires)
+        _tc_backward_sweep(lib, ts, B.cot_s, B.A, B.acts_s, P, m_dev, B.gs, B.gskip, ds.d_in)
         if dual:
             main.wait_stream(side)
         elif def_net is not None:
-            _tc_backward_sweep(lib, def_net, td, B.cot_d, B.A, B.acts_d, P, m_dev, B.gd, B.gskip,
-                               3 + 6 * dd.multires)
+            _tc_backward_sweep(lib, td, B.cot_d, B.A, B.acts_d, P, m_dev, B.gd, B.gskip, 3 + 6 * dd.multires)
         has_skip = any(l["skip"] for l in ts.layers)
         check(lib.sr_tc_trace_update(_p(idx), _p(m_dev), P, _p(pts), _p(B.gs), B.gs.shape[1],
                                      _p(B.gskip) if has_skip else None, B.gskip.shape[1],
@@ -1189,7 +1085,7 @@ def trace_surface_points_tc(sdf_net, def_net, lbs, cam_pos, rays, init_pts, batc
            lbs.ws_cl.data_ptr() if lbs is not None else 0, cp, float(dthreshold), float(athreshold),
            float(w1), float(w2), tuple(ds.pe_w[i] for i in range(ds.multires)),
            tuple(dd.pe_w[i] for i in range(dd.multires)) if dd is not None else (),
-           TC_REFINE_TRACE, TC_EPS_F, TC_EPS_A, TC_DUAL_STREAM, TC_SWEEP)
+           TC_REFINE_TRACE, TC_EPS_F, TC_EPS_A, TC_DUAL_STREAM)
     G = _tc_trace_ctx.get(key)
     if G is None:
         if len(_tc_trace_ctx) >= 4:
@@ -1236,30 +1132,6 @@ def trace_surface_points_tc(sdf_net, def_net, lbs, cam_pos, rays, init_pts, batc
         out = (G.pts.clone(), G.conv.clone())
         if return_counters:
             out = out + (G.counters.clone(),)
-    return out
-
-
-def _tc_layers_from_rows(lib, tcn, d_in, emb, ld, M, ch, n_out_last=None, skip_emb=None):
-    """embedded rows fp32 [M][ld] -> last layer outputs fp32 [M][n_last] on the tensor-core engine."""
-    dev = emb.device
-    A = torch.empty((lib.sr_tc_act_bytes(M, ld),), dtype=torch.uint8, device=dev)
-    check(lib.sr_tc_pack_rows(_p(emb), M, ld, ld, _p(A), None, _stream()), "tc_pack_rows")
-    K = ld
-    out = None
-    L = len(tcn.layers)
-    for i, ly in enumerate(tcn.layers):
-        last = i == L - 1
-        nxt = tcn.layers[i + 1] if not last else None
-        nv = ly["n"] if not (last and n_out_last) else n_out_last
-        Kn = _pad(nxt["k"], 32) if nxt else 0
-        skip_next = bool(nxt and nxt["skip"])
-        A_next = torch.empty((lib.sr_tc_act_bytes(M, Kn),), dtype=torch.uint8, device=dev) if nxt else None
-        o = torch.empty((M, nv), dtype=torch.float32, device=dev) if last else None
-        check(lib.sr_tc_linear(_p(A), _p(ly["W"]), _p(ly["bias"]), M, ly["n"], K, nv, ly["act"], ch, _p(A_next), Kn,
-                               0.7071067811865476 if skip_next else 1.0, _p(emb) if skip_next else None,
-                               d_in if skip_next else 0, ld, _p(o), nv if last else 0, 0, nv, None, None, 0, 0,
-                               1.0, None, _stream()), "tc_linear")
-        A, K, out = A_next, Kn, o
     return out
 
 
@@ -1311,5 +1183,7 @@ def shade_and_render_tc(sdf_full, def_net, lbs, render_net, pts, rays, batch_ind
         pw = (C.c_float * 16)(*[rd.pe_w[i] for i in range(16)])
         check(lib.sr_tc_render_embed(P, _p(pts), _p(crays), _p(normals), _p(s4), s4.shape[1], 1, nfeat, 4,
                                      rd.multires, pw, _p(emb), ld, _stream()), "tc_render_embed")
-        rgb = _tc_layers_from_rows(lib, tc_net(render_net), rd.d_in, emb, ld, P, 1)
+        rn = tc_net(render_net)
+        rgb = torch.empty((P, rn.layers[-1]["n"]), dtype=torch.float32, device=dev)
+        _tc_mlp(lib, rn, emb, 1, rgb)
     return normals, crays, rgb, dpos, ok

@@ -147,7 +147,7 @@ class TcMlpFunction(torch.autograd.Function):
             stashes = (C.c_void_p * max(L - 1, 1))(*[ar.ptr(o) if o is not None else None for o in o_st])
             out = torch.empty((M, Ws[-1].shape[0]), dtype=torch.float32, device=dev)
             check(lib.sr_tc_mlp_forward(layers, L, _p(x0), M, ld, cfg.d_in, ch, C.c_void_p(ar.ptr(o_in)), acts, stashes,
-                                        _p(out), _stream()), "tc_mlp_forward")
+                                        _p(out), None, 0, _stream()), "tc_mlp_forward")
             ops.LAUNCHES += L      # check() counted one; a sweep is 1 + L launches
         ctx.cfg, ctx.M, ctx.ld, ctx.L = cfg, M, ld, L
         ctx.arena, ctx.o_in, ctx.acts_c, ctx.stashes_c, ctx.o_act = ar, o_in, acts, stashes, o_act

@@ -1,81 +1,16 @@
-"""Host-side logic of the tensor-core engine that needs no GPU: how a chain of layer launches is split between the
-whole-sweep entry point (sr_tc_sweep) and per-layer calls (sr_tc_linear), and the struct layouts the C ABI reads."""
+"""Host-side logic that needs no GPU: the struct layouts the C ABI reads, the weight-norm helpers and the benchmark's
+parity report."""
 import ctypes as C
 
 import torch
 
-from selfreconcode_b200 import _lib, ops
-
-NONE, SOFTPLUS, RELU, TANH = 0, 1, 2, 3
-
-
-class FakeLib:
-    def __init__(self):
-        self.calls = []
-
-    def sr_tc_sweep(self, arr, n, M, ch, m_dev, stream):
-        self.calls.append(("sweep", n, [(arr[i].act, arr[i].mul_act, bool(arr[i].mul_tiles), arr[i].N, arr[i].K)
-                                        for i in range(n)]))
-        return 0
-
-    def sr_tc_linear(self, *a):
-        self.calls.append(("linear", a[4], a[5], a[7]))       # N, K, act
-        return 0
-
-
-def _chain(acts, mul=None, width=512, dstash_at=None):
-    t = torch.zeros(8)
-    steps = []
-    for i, a in enumerate(acts):
-        last = i == len(acts) - 1
-        kw = dict(A=t, W=t, bias=t, N=width if not last else 1, K=width, n_valid=width if not last else 1, act=a,
-                  A_next=None if last else t, K_next=0 if last else width, out=t if last else None)
-        if mul is not None and mul[i] is not None:
-            kw.update(mul_tiles=t, mul_K=width, mul_act=mul[i], act=NONE)
-        if dstash_at == i:
-            kw.update(dstash=t)
-        steps.append(ops._tc_step(**kw))
-    return steps
-
-
-def _run(monkeypatch, steps, sweep=True):
-    lib = FakeLib()
-    monkeypatch.setattr(ops, "_stream", lambda: C.c_void_p(0))
-    monkeypatch.setattr(ops, "TC_SWEEP", sweep)
-    n = ops._run_steps(lib, steps, 4096, 1, None)
-    return n, lib.calls
-
-
-def test_sweep_grouping(monkeypatch):
-    # SDF forward: eight softplus layers and the plain output layer -> one sweep of nine steps
-    n, calls = _run(monkeypatch, _chain([SOFTPLUS] * 8 + [NONE]))
-    assert n == 9 and [c[0] for c in calls] == ["sweep"] and calls[0][1] == 9
-    # renderer: ReLU layers + tanh head -> the ReLU run as a sweep, the head as its own launch
-    n, calls = _run(monkeypatch, _chain([RELU] * 4 + [TANH]))
-    assert n == 4 and [c[0] for c in calls] == ["sweep", "linear"] and calls[1][3] == TANH
-    # reverse sweep: act' multiplies on every step but the last (input gradient)
-    n, calls = _run(monkeypatch, _chain([NONE] * 9, mul=[SOFTPLUS] * 8 + [None]))
-    assert n == 9 and all(m for (_, _, m, _, _) in calls[0][2][:8]) and not calls[0][2][8][2]
-    # a training forward (fp32 act' stash requested) never takes the sweep entry point
-    n, calls = _run(monkeypatch, _chain([SOFTPLUS] * 3 + [NONE], dstash_at=0))
-    assert n == 0 and [c[0] for c in calls] == ["linear"] * 4
-    # unsupported activation first, or a single step: per-layer launches
-    assert _run(monkeypatch, _chain([TANH, TANH, NONE]))[0] == 0
-    assert _run(monkeypatch, _chain([NONE]))[0] == 0
-    # more than twelve steps do not fit the kernel's parameter block
-    assert _run(monkeypatch, _chain([RELU] * 13 + [NONE]))[0] == 0
-    # switched off: identical launches, one per layer
-    n, calls = _run(monkeypatch, _chain([SOFTPLUS] * 8 + [NONE]), sweep=False)
-    assert n == 0 and len(calls) == 9
-
+from selfreconcode_b200 import _lib
 
 def test_struct_layouts_match_header():
     """ctypes mirrors of the structs in include/selfrecon_b200.h: sizes follow from the field lists there
-    (8 pointers + 12 ints + 2 floats; 7 pointers + 4 ints; 4 pointers + 4 ints)."""
-    assert C.sizeof(_lib.TcStep) == 8 * 8 + 12 * 4 + 2 * 4
+    (7 pointers + 4 ints; 4 pointers + 4 ints)."""
     assert C.sizeof(_lib.WnLayer) == 7 * 8 + 4 * 4
     assert C.sizeof(_lib.TcLayer) == 4 * 8 + 4 * 4
-    assert _lib.TcStep.N.offset == 64 and _lib.TcStep.scale.offset == 112
     assert _lib.WnLayer.n.offset == 56
 
 
