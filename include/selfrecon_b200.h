@@ -268,7 +268,9 @@ int sr_shade_geometry(const sr_mlp_desc* sdf, const sr_mlp_desc* dnet, const sr_
  *                        tangents: tangent rows get act'(z_value) * acc, no bias);
  *                        A_next (tiled, K_next columns, may be NULL) receives scale*act(.) with
  *                        columns [n_valid, n_valid+skip_n) taken from skip_src (the skip concat of
- *                        network.py:88-89) and the rest zero; out (fp32 [M][out_ld], may be NULL)
+ *                        network.py:88-89) and the rest zero (K_next may exceed pad256(N): the
+ *                        chunks past it hold only skip / zero columns and are written by a second,
+ *                        small launch after the layer kernel); out (fp32 [M][out_ld], may be NULL)
  *                        receives result columns [out_col0, out_col0+out_n); dstash (fp32
  *                        [M][pad256(N)], may be NULL) receives act'(z) of value rows; mul_tiles
  *                        (may be NULL) switches the epilogue to the reverse-mode sweep
@@ -334,7 +336,7 @@ int sr_tc_unpack_rows(const void* T, int64_t M, int K, int Kpad, float* out, int
  * (acts[i], sr_tc_act_bytes(M, k_{i+1})) and, for softplus layers, the fp32 act'(z) (stashes[i] [M, pad256(n_i)] or
  * NULL).  m_dev (may be NULL): device-side row count <= M (active rays).  backward: gout [M, n_last] -> dW[l] [n,k] / db[l] [n] (NULL entries are
  * skipped) and x0_grad [M, ld] (or NULL); D0 / D1 = two delta tile buffers of sr_tc_act_bytes(M, widest layer),
- * part = sr_tc_wgrad_partial_bytes scratch for the widest pair, colsum_ws = colsum_slices x widest floats,
+ * part = sr_tc_wgrad_partial_bytes scratch, the largest over the layers' (Kd, Kx) pairs, colsum_ws = colsum_slices x widest floats,
  * g_skip [M, g_skip_ld] scratch when a layer has a skip connection. */
 typedef struct sr_tc_layer {
   const void* W;          /* packed weights, forward orientation (sr_tc_pack_weights of [n,k]) */

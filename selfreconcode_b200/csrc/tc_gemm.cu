@@ -46,7 +46,8 @@ struct LayerArgs {
   int skip_n, skip_ld;
   float* out;               // fp32 row-major [M][out_ld] (last layer), columns [0, n)
   int out_ld;
-  float* dstash;            // fp32 row-major [M][NT*256] act'(z) of value rows (reverse mode) or null
+  float* dstash;            // fp32 row-major act'(z) of value rows or null: written by a forward launch ([M][NT*256]),
+                            // read by a reverse launch ([M][pad256(n)], the previous layer's forward stash)
   // reverse sweep (MUL kernels): out = acc * act'(z_prev), act' recomputed from the previous layer's
   // stored output a (the tiles the forward pass wrote for this layer's input, scaled by 1/mul_inv_scale):
   // softplus100: 1 - exp(-100 a), relu: a > 0
@@ -155,10 +156,11 @@ __device__ __forceinline__ void epi_chunk(const LayerArgs& a, const EpiRow& r, u
       const __nv_bfloat16* mt = a.mul_tiles + a_tile_off(r.mt, c0 >> 5, a.mul_KC, 0) +
                                 (size_t)(r.row_in_tile >> 3) * 64 + (r.row_in_tile & 7) * 8;
       const float kk = -144.26950408889634f * a.mul_inv_scale;   // -100 log2(e) / scale
-      // optional fp32 act'(z) of the previous layer's VALUE rows (written by its forward launch as `dstash`)
-      // rows past M read row 0's entries (discarded below)
+      // optional fp32 act'(z) of the previous layer's VALUE rows (written by its forward launch as `dstash`, row
+      // pitch pad256(n)); only chunks with columns < n use act', the skip columns of a skip layer's input have none.
+      // Rows past M read row 0's entries (discarded below)
       const long long srow = r.row_ok ? (CH == 4 ? (r.row & ~3LL) : r.row) : 0;
-      const float* stash = a.dstash == nullptr ? nullptr : a.dstash + (size_t)srow * r.ds_ld + c0;
+      const float* stash = a.dstash == nullptr || c0 >= a.n ? nullptr : a.dstash + (size_t)srow * r.ds_ld + c0;
       const bool use_stash = (ACT == SR_ACT_SOFTPLUS100) && stash != nullptr;
       // PF: all global operands of the chunk first (8 x 16 B of activation tiles, 8 x 16 B of stash), 16 loads in
       // flight per thread; PF = false requests them per group of 8 columns (fewer registers)
@@ -416,7 +418,9 @@ __global__ void __launch_bounds__(kThreads, 1) tc_sweep_kernel(const __grid_cons
     r.row_in_tile = cw * 64 + (wq & 1) * 32 + lane;
     r.lane = lane;
     r.is_val = (CH == 1) || ((lane & 3) == 0);
-    r.ds_ld = (size_t)a.NT * BN;
+    // act' stash pitch: a forward launch writes pad256(N); a reverse launch reads the previous layer's stash, whose
+    // width is this launch's n (N = n + d_in for a skip layer, which may cross a multiple of 256)
+    r.ds_ld = MUL ? (size_t)((a.n + BN - 1) / BN) * BN : (size_t)a.NT * BN;
     int slot = 0;
     uint32_t phase = 0;
     for (int j = 0; j < J; ++j) {
@@ -509,6 +513,43 @@ __global__ void pack_rows_kernel(const float* __restrict__ src, long long M, int
     *reinterpret_cast<uint4*>(dst + a_tile_off(mt, kc, KC, 1) + off) = *reinterpret_cast<uint4*>(p2);
     if constexpr (kPlanes == 3)
       *reinterpret_cast<uint4*>(dst + a_tile_off(mt, kc, KC, kPlanes - 1) + off) = *reinterpret_cast<uint4*>(p3);
+  }
+}
+
+// k chunks [kc0, KCn) of a layer's next-layer tiles that lie past its last column tile, which the layer kernel's
+// epilogue never reaches: a skip layer's input n + skip_n can be wider than pad256(n).  scale * skip_src in columns
+// [n, n + skip_n), zero elsewhere and in rows past the (device-side) row count, as the epilogue writes them.
+__global__ void pack_skip_tail_kernel(const float* __restrict__ skip_src, int skip_ld, int n, int skip_n, float scale,
+                                      long long M, int kc0, int KCn, __nv_bfloat16* __restrict__ dst,
+                                      const int* __restrict__ m_dev) {
+  if (m_dev != nullptr) {
+    const long long md = *m_dev;
+    M = md < M ? md : M;
+  }
+  const long long MT = (M + BM - 1) / BM;
+  const int nkc = KCn - kc0;
+  const long long total = MT * BM * (long long)nkc * 4;  // one thread per (row, k8 group)
+  for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
+       idx += (long long)gridDim.x * blockDim.x) {
+    const int r = (int)(idx % BM);
+    const long long rest = idx / BM;
+    const int g = (int)(rest % (nkc * 4));
+    const long long mt = rest / (nkc * 4);
+    const long long row = mt * BM + r;
+    const int kc = kc0 + (g >> 2), k8 = g & 3;
+    __align__(16) __nv_bfloat16 p1[8], p2[8], p3[8];
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      const int c = kc * 32 + k8 * 8 + e;
+      const float x = (skip_src != nullptr && row < M && c >= n && c < n + skip_n)
+                          ? skip_src[(size_t)row * skip_ld + (c - n)] * scale : 0.f;
+      split3(x, p1[e], p2[e], p3[e]);
+    }
+    const size_t off = (size_t)k8 * (BM * 8) + (size_t)(r >> 3) * 64 + (r & 7) * 8;
+    *reinterpret_cast<uint4*>(dst + a_tile_off(mt, kc, KCn, 0) + off) = *reinterpret_cast<uint4*>(p1);
+    *reinterpret_cast<uint4*>(dst + a_tile_off(mt, kc, KCn, 1) + off) = *reinterpret_cast<uint4*>(p2);
+    if constexpr (kPlanes == 3)
+      *reinterpret_cast<uint4*>(dst + a_tile_off(mt, kc, KCn, kPlanes - 1) + off) = *reinterpret_cast<uint4*>(p3);
   }
 }
 
@@ -679,7 +720,9 @@ int sr_tc_pack_weights(const float* w, int N, int K, int ld, void* dst, cudaStre
   return sr_launch_status();
 }
 
-// picks the instantiation for (activation, mode, ch) and launches one CTA per row tile, at most one per SM
+// picks the instantiation for (activation, mode, ch) and launches one CTA per row tile, at most one per SM; when the
+// next layer's input is wider than pad256(N) (a skip layer's n + skip_n), pack_skip_tail_kernel writes the chunks past
+// the last column tile in a second launch
 int sr_tc_linear(const void* A, const void* W, const float* bias, int64_t M, int N, int K, int n_valid,
                  int act, int ch, void* A_next, int K_next, float scale, const float* skip_src,
                  int skip_n, int skip_ld, float* out, int out_ld, int out_col0, int out_n,
@@ -735,6 +778,14 @@ int sr_tc_linear(const void* A, const void* W, const float* bias, int64_t M, int
   }
   const int grid = a.MT < SR_NUM_SMS ? a.MT : SR_NUM_SMS;
   kern<<<grid, kThreads, kSmem, s>>>(a);
+  const int kc0 = a.NT * (BN / 32);   // first next-layer chunk the epilogue does not produce
+  if (a.A_next != nullptr && a.KCn > kc0) {
+    const int rc = sr_launch_status();
+    if (rc) return rc;
+    const long long total = (long long)a.MT * BM * (a.KCn - kc0) * 4;
+    pack_skip_tail_kernel<<<sr_grid_for(total, 256, 8), 256, 0, s>>>(a.skip_src, a.skip_ld, a.n, a.skip_n, a.scale, M,
+                                                                     kc0, a.KCn, a.A_next, m_dev);
+  }
   return sr_launch_status();
 }
 }

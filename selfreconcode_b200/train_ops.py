@@ -169,11 +169,13 @@ class TcMlpFunction(torch.autograd.Function):
         with torch.cuda.device(dev):
             g = gout.detach().contiguous().float()
             wmax = max(_pad(n, 32) for n, _ in shapes)
-            kmax = max([_pad(k, 32) for _, k in shapes[1:]] + [ld])
             ar = _Arena(dev)
             o_d0 = ar.add(lib.sr_tc_act_bytes(M, wmax))[1]
             o_d1 = ar.add(lib.sr_tc_act_bytes(M, wmax))[1]
-            o_part = ar.add(lib.sr_tc_wgrad_partial_bytes(M, wmax, kmax, None))[1]
+            # the split count grows as a layer's dW tiles shrink: a narrower pair can need more scratch than the widest
+            kxs = [ld] + [_pad(k, 32) for _, k in shapes[1:]]
+            o_part = ar.add(max(lib.sr_tc_wgrad_partial_bytes(M, _pad(n, 32), kx, None)
+                                for (n, _), kx in zip(shapes, kxs)))[1]
             o_cs = ar.add(COLSUM_SLICES * wmax * 4)[1]
             gs_ld = _pad(cfg.d_in, 4)
             o_gs = ar.add(M * gs_ld * 4)[1] if any(cfg.skips) else None
