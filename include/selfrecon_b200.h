@@ -310,6 +310,28 @@ int sr_tc_linear(const void* A, const void* W, const float* bias, int64_t M, int
 int sr_raster_mesh(const float* verts_screen, const int64_t* faces, int64_t N, int64_t V, int64_t F, int H, int W,
                    uint64_t* keys, int64_t* pix_to_face, float* bary, float* zbuf, cudaStream_t s);
 
+/* Shaded images of OptimNetwork.infer (model/network.py:318-338 with infer.py:90's HardPhongShader), forward only.
+ * sr_mesh_vertex_normals: pytorch3d's Meshes.verts_normals_packed for N frames of world vertices [N,V,3] sharing one
+ *   face table [F,3]: the sum of the unnormalised face normals (v2-v1) x (v0-v1) over the incident faces, divided by
+ *   max(|sum|, 1e-6).  vf_offsets [V+1] / vf_faces = CSR of each vertex's incident faces in ascending order; the sum
+ *   follows that order (no atomics: bit-identical reruns).  normals [N,V,3].
+ * sr_shade_phong: pytorch3d's phong_shading + hard_rgb_blend with faces_per_pixel = 1, one point light and one
+ *   material, on the fragments sr_raster_mesh writes (pix_to_face [N,H,W] = n*F + f or -1, bary [N,H,W,3]).
+ *   verts / normals / colors [N,V,3] (colors NULL = white), cam_pos / light_pos [N,3] device arrays (per image frame).
+ *   out [N,H,W,4] (16-byte aligned): (rgb, 1) on covered pixels, (background, 0) elsewhere. */
+typedef struct sr_phong_params {
+  float light_ambient[3], light_diffuse[3], light_specular[3];
+  float mat_ambient[3], mat_diffuse[3], mat_specular[3];
+  float shininess;
+  float background[3];
+} sr_phong_params;
+int sr_mesh_vertex_normals(const float* verts, const int64_t* faces, const int64_t* vf_offsets, const int64_t* vf_faces,
+                           int64_t N, int64_t V, int64_t F, float* normals, cudaStream_t s);
+int sr_shade_phong(const float* verts, const float* normals, const float* colors, const int64_t* faces, int64_t N,
+                   int64_t V, int64_t F, const int64_t* pix_to_face, const float* bary, int H, int W,
+                   const float* cam_pos, const float* light_pos, const sr_phong_params* params, float* out,
+                   cudaStream_t s);
+
 /* Training half of the tensor-core engine (model/network.py:599-639, 774-796: loss.backward() and the parameter
  * VJPs; in a reverse launch (`mul_tiles` != NULL) `dstash` is an INPUT: the fp32 act'(z) the forward launch of the
  * previous layer wrote (leading dimension = that layer's width rounded up to 256), or NULL to recompute act' from the

@@ -57,6 +57,13 @@ class TraceParams(C.Structure):
                 ("w1", C.c_float), ("w2", C.c_float)]
 
 
+class PhongParams(C.Structure):
+    """struct sr_phong_params (light / material colours of sr_shade_phong)."""
+    _fields_ = [("light_ambient", C.c_float * 3), ("light_diffuse", C.c_float * 3), ("light_specular", C.c_float * 3),
+                ("mat_ambient", C.c_float * 3), ("mat_diffuse", C.c_float * 3), ("mat_specular", C.c_float * 3),
+                ("shininess", C.c_float), ("background", C.c_float * 3)]
+
+
 # name -> (restype, argtypes); every symbol include/selfrecon_b200.h declares
 SIGNATURES = {
     "sr_abi_version": (C.c_int, []),
@@ -118,6 +125,9 @@ SIGNATURES = {
     "sr_tc_trace_update": (C.c_int, [c_f, c_f, i64, c_f, c_f, i32, c_f, i32, c_f, i32, c_f, i32,
                                      C.POINTER(f32), i32, C.POINTER(f32), c_f, c_f, c_f, stream_t]),
     "sr_raster_mesh": (C.c_int, [c_f, c_f, i64, i64, i64, i32, i32, c_f, c_f, c_f, c_f, stream_t]),
+    "sr_mesh_vertex_normals": (C.c_int, [c_f, c_f, c_f, c_f, i64, i64, i64, c_f, stream_t]),
+    "sr_shade_phong": (C.c_int, [c_f, c_f, c_f, c_f, i64, i64, i64, c_f, c_f, i32, i32, c_f, c_f,
+                                 C.POINTER(PhongParams), c_f, stream_t]),
     "sr_tc_wgrad_partial_bytes": (i64, [i64, i32, i32, C.POINTER(C.c_int)]),
     "sr_tc_debug_wgrad_desc_swap": (None, [i32]),
     "sr_tc_mlp_forward": (C.c_int, [C.POINTER(TcLayer), i32, c_f, i64, i32, i32, i32, c_f, C.POINTER(C.c_void_p),

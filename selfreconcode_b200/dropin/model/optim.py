@@ -412,9 +412,12 @@ class OptimNetwork(nn.Module):
             if isinstance(r, dict):
                 return r['batch_inds'], r['row_inds'], r['col_inds'], r['initTmpPs'], r.get('front_face_ids')
             return utils.FindSurfacePs(TmpVs.detach(), Tmpfs, r)
-        from .raster import SilhouetteRenderer
+        from .raster import MeshRenderer, SilhouetteRenderer
         if isinstance(self.maskRender, SilhouetteRenderer):      # built-in device rasteriser (csrc/raster.cu)
             _, frags = self.maskRender(defTmpVs.detach(), Tmpfs)
+            return utils.FindSurfacePs(TmpVs.detach(), Tmpfs, frags)
+        if isinstance(self.maskRender, MeshRenderer):            # same rasteriser; the seed needs no shading
+            frags = self.maskRender.rasterizer(defTmpVs.detach(), Tmpfs)
             return utils.FindSurfacePs(TmpVs.detach(), Tmpfs, frags)
         P = _p3d()
         meshes = P.Meshes(verts=[v.view(V, 3) for v in torch.split(defTmpVs.detach(), 1)], faces=[Tmpfs] * N)
@@ -552,9 +555,13 @@ class OptimNetwork(nn.Module):
 
     # ---- network.py:306-372 ---------------------------------------------------------------------
     def infer(self, TmpVs, Tmpfs, H, W, ratio, frame_ids, notcolor=False, gts=None):
-        """Renders N frames: silhouette shading of the deformed and of the translator-only template
-        (pytorch3d mesh renderer), then the neural colour of every covered pixel through infer_rays.
-        -> (colors uint8 [N,H,W,3] | None, imgs, def1imgs, deformed vertices)."""
+        """Renders N frames: shaded images of the deformed and of the translator-only template (whatever shader
+        maskRender holds), then the neural colour of every covered pixel through infer_rays.
+        -> (colors uint8 [N,H,W,3] | None, imgs, def1imgs, deformed vertices).
+        With a built-in renderer (raster.SilhouetteRenderer / raster.MeshRenderer) no pytorch3d is needed."""
+        from .raster import MeshRenderer, SilhouetteRenderer
+        if isinstance(self.maskRender, (SilhouetteRenderer, MeshRenderer)):
+            return self._infer_builtin(TmpVs, Tmpfs, ratio, frame_ids, notcolor, gts)
         device = TmpVs.device
         P = _p3d()
         N, V = frame_ids.numel(), TmpVs.shape[0]
@@ -587,6 +594,48 @@ class OptimNetwork(nn.Module):
             cam1 = type(cameras)(focals, pps, front, newTs.repeat(N, 1), image_size=[(W, H)]).to(device)
             def1imgs, _ = self.maskRender(meshes1, cameras=cam1,
                                           lights=P.PointLights(device=device, location=((0, 1, newTs[0, 2].item()),)))
+            def1imgs = torch.clamp(def1imgs * 255., min=0., max=255.).cpu().numpy().astype(np.uint8)
+            bi, ri, ci, ps, _ = utils.FindSurfacePs(TmpVs.detach(), Tmpfs, frags)
+        if notcolor:
+            return None, imgs, def1imgs, defMeshVs
+        print('draw %d points' % bi.shape[0])
+        colors = self.infer_rays(bi, ri, ci, ps, H, W, ratio, frame_ids)
+        if gts and 'image' in gts and masks is not None:
+            colors[~masks] = gts['image'][~masks][:, :3] * 255.
+        return colors.cpu().numpy().astype(np.uint8), imgs, def1imgs, defMeshVs
+
+    def _infer_builtin(self, TmpVs, Tmpfs, ratio, frame_ids, notcolor, gts):
+        """infer() on the built-in renderer: the same sequence (network.py:306-372) with the device rasteriser and,
+        for a MeshRenderer, the device Phong shader (csrc/mesh_shade.cu) in place of pytorch3d's Meshes pipeline."""
+        from .raster import PointLights
+        device = TmpVs.device
+        N = frame_ids.numel()
+        with torch.no_grad():
+            cameras, H, W = self._cameras(N, device)
+            self.maskRender.rasterizer.cameras = cameras
+            if self.pcRender is not None:
+                self.pcRender.rasterizer.cameras = cameras
+            poses, trans, d_cond, _ = self.dataset.get_grad_parameters(frame_ids, device)
+            defTmpVs = self.deformer(TmpVs[None].expand(N, -1, 3), [d_cond, [poses, trans]], ratio=ratio)
+            defMeshVs = defTmpVs.detach().cpu().numpy()
+            imgs, frags = self.maskRender(defTmpVs.detach(), Tmpfs)
+            masks = None
+            if gts:
+                m = (frags.pix_to_face >= 0).float()[..., 0]
+                g = gts['mask']
+                gts['maskE'] = (1. - (m * g).view(N, -1).sum(1) / (m + g - m * g).abs().view(N, -1).sum(1)).cpu().numpy()
+                masks = m > 0.
+                imgs = imgs[..., :3]
+                if 'image' in gts:
+                    imgs[~masks] = gts['image'][~masks][:, [2, 1, 0]]
+            imgs = torch.clamp(imgs * 255., min=0., max=255.).cpu().numpy().astype(np.uint8)
+            d1 = self.deformer.defs[0](TmpVs[None].expand(N, -1, 3), d_cond, ratio=ratio)
+            newTs = self.dataset.trans.mean(0).to(device)[None, :]
+            front = torch.tensor([[[-1., 0., 0.], [0., 1., 0.], [0., 0., -1.]]], device=device).repeat(N, 1, 1)
+            focals, pps, _, _, _, _ = self.dataset.get_camera_parameters(N, device)
+            cam1 = type(cameras)(focals, pps, front, newTs.repeat(N, 1), image_size=[(W, H)]).to(device)
+            def1imgs, _ = self.maskRender(d1.detach(), Tmpfs, cameras=cam1,
+                                          lights=PointLights(device=device, location=((0, 1, newTs[0, 2].item()),)))
             def1imgs = torch.clamp(def1imgs * 255., min=0., max=255.).cpu().numpy().astype(np.uint8)
             bi, ri, ci, ps, _ = utils.FindSurfacePs(TmpVs.detach(), Tmpfs, frags)
         if notcolor:

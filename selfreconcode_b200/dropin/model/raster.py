@@ -5,12 +5,14 @@ behind `optNet.maskRender.rasterizer`): it owns `.cameras` and `.raster_settings
 into Fragments(pix_to_face, bary_coords, zbuf) -- on one CUDA kernel pair (csrc/raster.cu) instead of the
 binned pytorch3d pipeline, and on the camera convention of RectifiedPerspectiveCameras.project directly
 (pixel centres at integer (col, row)), so no NDC round trip.  `SilhouetteRenderer` is the minimal
-MeshRendererWithFragments: `renderer(verts [N,V,3], faces) -> (hard silhouette [N,H,W,4], fragments)`."""
+MeshRendererWithFragments: `renderer(verts [N,V,3], faces) -> (hard silhouette [N,H,W,4], fragments)`.
+`MeshRenderer` with `HardPhongShader` is the shaded counterpart OptimNetwork.infer renders with (infer.py:80-90):
+Phong-lit images of the same fragments (csrc/mesh_shade.cu)."""
 import types
 
 import torch
 
-from selfreconcode_b200 import ops
+from selfreconcode_b200 import _lib, ops
 
 
 class RasterSettings:
@@ -72,3 +74,136 @@ class SilhouetteRenderer:
         frags = self.rasterizer(verts, faces, cameras)
         cover = (frags.pix_to_face >= 0).float()
         return torch.cat([cover.expand(-1, -1, -1, 3), cover], dim=-1), frags
+
+
+# ---- shaded images of OptimNetwork.infer (model/network.py:318-338; infer.py:90 installs HardPhongShader) ---------
+# The classes below take pytorch3d's keyword names and defaults (pytorch3d.renderer PointLights, Materials,
+# BlendParams, HardPhongShader); the shading itself is csrc/mesh_shade.cu.  Forward only, one face per pixel.
+
+def _rgb(c, what):
+    """A colour argument ((r, g, b),) / (r, g, b) / tensor -> 3 host floats (one colour for every frame)."""
+    t = torch.as_tensor(c, dtype=torch.float64).detach().cpu().reshape(-1, 3)
+    if not bool((t == t[:1]).all()):
+        raise NotImplementedError("%s: one colour for all frames is supported, got %d different ones" % (what, t.shape[0]))
+    return tuple(float(x) for x in t[0])
+
+
+class PointLights:
+    def __init__(self, device=None, location=((0., 1., 0.),), ambient_color=((0.5, 0.5, 0.5),),
+                 diffuse_color=((0.3, 0.3, 0.3),), specular_color=((0.2, 0.2, 0.2),)):
+        self.device = device
+        self.location = torch.as_tensor(location, dtype=torch.float32, device=device).reshape(-1, 3)
+        self.ambient_color = _rgb(ambient_color, "PointLights.ambient_color")
+        self.diffuse_color = _rgb(diffuse_color, "PointLights.diffuse_color")
+        self.specular_color = _rgb(specular_color, "PointLights.specular_color")
+
+    def to(self, device):
+        self.device = device
+        self.location = self.location.to(device)
+        return self
+
+
+class Materials:
+    def __init__(self, device=None, ambient_color=((1., 1., 1.),), diffuse_color=((1., 1., 1.),),
+                 specular_color=((1., 1., 1.),), shininess=64):
+        self.device = device
+        self.ambient_color = _rgb(ambient_color, "Materials.ambient_color")
+        self.diffuse_color = _rgb(diffuse_color, "Materials.diffuse_color")
+        self.specular_color = _rgb(specular_color, "Materials.specular_color")
+        s = torch.as_tensor(shininess, dtype=torch.float64).reshape(-1)
+        if not bool((s == s[:1]).all()):
+            raise NotImplementedError("Materials.shininess: one value for all frames is supported")
+        self.shininess = float(s[0])
+
+    def to(self, device):
+        self.device = device
+        return self
+
+
+class BlendParams:
+    def __init__(self, sigma=1e-4, gamma=1e-4, background_color=(1., 1., 1.)):
+        self.sigma = sigma
+        self.gamma = gamma
+        self.background_color = tuple(float(x) for x in torch.as_tensor(background_color).reshape(3).tolist())
+
+
+def vertex_face_csr(faces, n_verts):
+    """(offsets [V+1], incident face ids) of every vertex, faces ascending per vertex: one stable device sort of the
+    face table (optim.vertex_face_pairs) plus a binary search for the offsets (no atomics)."""
+    from .optim import vertex_face_pairs
+    vid, fid = vertex_face_pairs(faces, n_verts)
+    offsets = torch.searchsorted(vid, torch.arange(n_verts + 1, device=vid.device, dtype=vid.dtype))
+    return offsets, fid
+
+
+class HardPhongShader:
+    """`images = shader(fragments, verts [N,V,3], faces, ...)`: per-pixel Phong lighting of the interpolated position,
+    vertex normal and per-vertex colour (white when none is given), hard blend over the background."""
+
+    def __init__(self, device=None, cameras=None, lights=None, materials=None, blend_params=None):
+        self.cameras = cameras
+        self.lights = lights if lights is not None else PointLights(device=device)
+        self.materials = materials if materials is not None else Materials(device=device)
+        self.blend_params = blend_params if blend_params is not None else BlendParams()
+        self._csr = None    # (faces, faces._version, V, csr): the CSR is built once per mesh
+
+    def to(self, device):
+        if hasattr(self.cameras, "to"):
+            self.cameras = self.cameras.to(device)
+        self.lights.to(device)
+        self.materials.to(device)
+        return self
+
+    def csr(self, faces, n_verts):
+        c = self._csr
+        if c is None or c[0] is not faces or c[1] != faces._version or c[2] != n_verts:
+            self._csr = (faces, faces._version, n_verts, vertex_face_csr(faces, n_verts))
+        return self._csr[3]
+
+    def params(self, lights, materials, blend_params):
+        p = _lib.PhongParams()
+        for field, val in (("light_ambient", lights.ambient_color), ("light_diffuse", lights.diffuse_color),
+                           ("light_specular", lights.specular_color), ("mat_ambient", materials.ambient_color),
+                           ("mat_diffuse", materials.diffuse_color), ("mat_specular", materials.specular_color),
+                           ("background", blend_params.background_color)):
+            getattr(p, field)[:] = val
+        p.shininess = materials.shininess
+        return p
+
+    def __call__(self, fragments, verts, faces, cameras=None, lights=None, materials=None, blend_params=None,
+                 verts_colors=None, **kwargs):
+        cam = cameras if cameras is not None else self.cameras
+        if cam is None:
+            raise ValueError("HardPhongShader needs cameras (constructor or call argument)")
+        lights = lights if lights is not None else self.lights
+        materials = materials if materials is not None else self.materials
+        blend_params = blend_params if blend_params is not None else self.blend_params
+        N, V = verts.shape[0], verts.shape[1]
+        with torch.no_grad():
+            vs = verts.detach().contiguous().float()
+            normals = ops.mesh_vertex_normals(vs, faces, self.csr(faces, V))       # all N frames in one launch
+            R, T = cam.R[:N], cam.T[:N]
+            cam_pos = -(R * T.view(N, 1, 3)).sum(2)          # cameras.cam_pos(n) for every frame, no host sync
+            light_pos = lights.location.to(vs.device).expand(N, 3)
+            return ops.shade_phong(vs, normals, faces, fragments.pix_to_face, fragments.bary_coords, cam_pos,
+                                   light_pos, self.params(lights, materials, blend_params), colors=verts_colors)
+
+
+class MeshRenderer:
+    """Built-in counterpart of pytorch3d's MeshRendererWithFragments:
+    `images [N,H,W,4], fragments = renderer(verts [N,V,3], faces, cameras=None, lights=None)`; `cameras` overrides
+    both the rasteriser's and the shader's cameras for this call, `lights` the shader's lights."""
+
+    def __init__(self, rasterizer, shader):
+        self.rasterizer = rasterizer
+        self.shader = shader
+
+    def to(self, device):
+        self.rasterizer.to(device)
+        self.shader.to(device)
+        return self
+
+    def __call__(self, verts, faces, cameras=None, lights=None, **kwargs):
+        frags = self.rasterizer(verts, faces, cameras)
+        images = self.shader(frags, verts, faces, cameras=cameras, lights=lights, **kwargs)
+        return images, frags

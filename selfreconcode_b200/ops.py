@@ -110,6 +110,52 @@ def raster_mesh(verts_screen, faces, H, W):
 _KERNELS_PER_CALL["raster_mesh"] = 2
 
 
+def mesh_vertex_normals(verts, faces, csr):
+    """verts [N,V,3] world positions of N frames sharing faces [F,3] int64; csr = (offsets [V+1], face ids) of each
+    vertex's incident faces, ascending -> [N,V,3] pytorch3d vertex normals (area-weighted, F.normalize eps 1e-6)."""
+    _need_cuda(verts, faces, csr[0], csr[1])
+    vs = verts.detach().contiguous().float()
+    fc = faces.contiguous().to(torch.int64)
+    off, fid = csr[0].contiguous().to(torch.int64), csr[1].contiguous().to(torch.int64)
+    N, V, _ = vs.shape
+    if off.numel() != V + 1:
+        raise ValueError("mesh_vertex_normals: csr offsets must have V + 1 entries")
+    out = torch.empty_like(vs)
+    with torch.cuda.device(vs.device):
+        check(_lib.load().sr_mesh_vertex_normals(_p(vs), _p(fc), _p(off), _p(fid), N, V, fc.shape[0], _p(out),
+                                                 _stream()), "mesh_vertex_normals")
+    return out
+
+
+def shade_phong(verts, normals, faces, pix_to_face, bary, cam_pos, light_pos, params, colors=None):
+    """pytorch3d HardPhongShader (phong_shading + hard_rgb_blend, one face per pixel) on rasteriser fragments.
+    verts / normals / colors [N,V,3] (colors None = white), pix_to_face [N,H,W(,1)] packed ids, bary [N,H,W(,1),3],
+    cam_pos / light_pos [N,3] device tensors, params a _lib.PhongParams -> images [N,H,W,4]."""
+    _need_cuda(verts, normals, faces, pix_to_face, bary, cam_pos, light_pos, colors)
+    vs = verts.detach().contiguous().float()
+    N, V, _ = vs.shape
+    H, W = pix_to_face.shape[1], pix_to_face.shape[2]
+    nr = normals.detach().contiguous().float()
+    col = colors.detach().contiguous().float() if colors is not None else None
+    fc = faces.contiguous().to(torch.int64)
+    p2f = pix_to_face.contiguous().to(torch.int64)
+    br = bary.detach().contiguous().float()
+    cp = cam_pos.detach().float().reshape(-1, 3).expand(N, 3).contiguous()
+    lp = light_pos.detach().float().reshape(-1, 3).expand(N, 3).contiguous()
+    if nr.shape != vs.shape or (col is not None and col.shape != vs.shape) or p2f.numel() != N * H * W \
+            or br.numel() != 3 * N * H * W:
+        raise ValueError("shade_phong: inconsistent shapes")
+    out = torch.empty((N, H, W, 4), dtype=torch.float32, device=vs.device)
+    with torch.cuda.device(vs.device):
+        check(_lib.load().sr_shade_phong(_p(vs), _p(nr), _p(col), _p(fc), N, V, fc.shape[0], _p(p2f), _p(br),
+                                         int(H), int(W), _p(cp), _p(lp), C.byref(params), _p(out), _stream()),
+              "shade_phong")
+    return out
+
+
+_KERNELS_PER_CALL.update({"mesh_vertex_normals": 1, "shade_phong": 1})
+
+
 def svals3x3(J, want_v=True):
     """J [n,3,3] f32 CUDA -> (singular values [n,3] descending, V [n,3,3] | None)."""
     _need_cuda(J)
