@@ -262,7 +262,8 @@ int sr_shade_geometry(const sr_mlp_desc* sdf, const sr_mlp_desc* dnet, const sr_
  * tile layout of the wgmma descriptors (see csrc/tc_gemm.cu):
  *   sr_tc_act_bytes(M,K) / sr_tc_weight_bytes(N,K): buffer sizes of tiled activations / weights
  *   sr_tc_pack_rows    : fp32 row-major [M][K] (ld) -> tiled split-bf16 activations
- *   sr_tc_pack_weights : fp32 row-major [N][K] (ld) effective weights -> tiled split-bf16
+ *   sr_tc_pack_weights : fp32 row-major [N][K] (ld) effective weights -> tiled split-bf16 (64-column
+ *                        tiles when N <= 64, else 256: a pack is only valid for launches of the same N)
  *   sr_tc_linear       : one layer. A (tiled, K), W (tiled, N x K), bias [pad256(N)];
  *                        n_valid output columns; ch = rows per point (1, or 4 = value + 3
  *                        tangents: tangent rows get act'(z_value) * acc, no bias);
@@ -289,9 +290,10 @@ int sr_tc_embed(const float* pts, int64_t P, int multires, const float* pe_w, in
                 float* out, int ld, const int32_t* index /* optional active list */,
                 const int32_t* m_dev /* optional device-side count */, cudaStream_t s);
 /* Backward of sr_tc_embed w.r.t. the points: gx [P*ch, ld] -> gp [P,3] (value row: d PE/dp; tangent rows: second
- * derivative of the encoding).  The latent-code columns are a plain slice of gx (value rows). multires <= 8. */
+ * derivative of the encoding).  The latent-code columns are a plain slice of gx (value rows). multires <= 8.
+ * gk [P, gk_ld] (ch = 1 only, or NULL) is added to gx's encoding columns: a skip layer's part of a reverse sweep. */
 int sr_tc_embed_backward(const float* pts, int64_t P, int multires, const float* pe_w, int ch, const float* gx, int ld,
-                         float* gp, cudaStream_t s);
+                         const float* gk, int gk_ld, float* gp, cudaStream_t s);
 int64_t sr_tc_act_bytes(int64_t M, int K);
 int64_t sr_tc_weight_bytes(int N, int K);
 int sr_tc_pack_rows(const float* src, int64_t M, int K, int ld, void* dst, const int32_t* m_dev,
@@ -432,13 +434,13 @@ int sr_tc_trace_update(const int32_t* index, const int32_t* m_dev, int64_t P, fl
                        const float* pw_d, int32_t* active_out, int32_t* counter_out,
                        const uint8_t* converged /* or NULL */, cudaStream_t s);
 
-/* Shading on the tensor-core engine: sr_tc_shade_point turns the 4-rows-per-point outputs of the
- * SDF (value / grad f in column 0) and translator (offset / d offset) sweeps into normals,
- * cardinal rays (J^-1 v, fallback v when |det J| < 1e-4) and D(p); sr_tc_render_embed builds
+/* Shading on the tensor-core engine: sr_tc_shade_point turns grad f [P,3] (the SDF's reverse sweep
+ * through sr_tc_embed_backward) and the 4-rows-per-point translator outputs (offset / d offset) into
+ * normals, cardinal rays (J^-1 v, fallback v when |det J| < 1e-4) and D(p); sr_tc_render_embed builds
  * cat([p, PE(view), n, feat]) rows for the rendering network (RenderNet.py:73-74); feat is read
  * from row p*feat_row_stride of a [*, feat_ld] matrix starting at column feat_col0. */
 int sr_tc_shade_point(int64_t P, const float* pts, const float* rays, const int64_t* batch_inds,
-                      const float* sdf4, int ld_s, const float* off4, const sr_lbs_params* lbs,
+                      const float* grad, const float* off4, const sr_lbs_params* lbs,
                       float* normals, float* crays, float* dpos, uint8_t* inv_ok, cudaStream_t s);
 int sr_tc_render_embed(int64_t P, const float* pts, const float* views, const float* normals,
                        const float* feat, int feat_ld, int feat_col0, int nfeat, int feat_row_stride,

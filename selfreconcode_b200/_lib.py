@@ -112,7 +112,7 @@ SIGNATURES = {
                                     stream_t]),
     "sr_tc_embed": (C.c_int, [c_f, i64, i32, C.POINTER(f32), i32, c_f, c_f, i64, i32, c_f, i32, c_f, c_f,
                               stream_t]),
-    "sr_tc_embed_backward": (C.c_int, [c_f, i64, i32, C.POINTER(f32), i32, c_f, i32, c_f, stream_t]),
+    "sr_tc_embed_backward": (C.c_int, [c_f, i64, i32, C.POINTER(f32), i32, c_f, i32, c_f, i32, c_f, stream_t]),
     "sr_tc_act_bytes": (i64, [i64, i32]),
     "sr_tc_weight_bytes": (i64, [i32, i32]),
     "sr_tc_pack_rows": (C.c_int, [c_f, i64, i32, i32, c_f, c_f, stream_t]),
@@ -146,8 +146,8 @@ SIGNATURES = {
     "sr_sdf_small_work_bytes": (i64, [i32]),
     "sr_sdf_forward_small": (C.c_int, [C.POINTER(MlpDesc), c_f, i64, c_f, c_f, c_f, c_f, i32, stream_t]),
     "sr_sdf_forward_indexed": (C.c_int, [C.POINTER(MlpDesc), c_f, i64, c_f, c_f, c_f, stream_t]),
-    "sr_tc_shade_point": (C.c_int, [i64, c_f, c_f, c_f, c_f, i32, c_f, C.POINTER(LbsParams), c_f, c_f, c_f,
-                                    c_f, stream_t]),
+    "sr_tc_shade_point": (C.c_int, [i64, c_f, c_f, c_f, c_f, c_f, C.POINTER(LbsParams), c_f, c_f, c_f, c_f,
+                                    stream_t]),
     "sr_tc_render_embed": (C.c_int, [i64, c_f, c_f, c_f, c_f, i32, i32, i32, i32, i32, C.POINTER(f32), c_f,
                                      i32, stream_t]),
     "sr_seg3d_candidates": (C.c_int, [c_f, c_f, c_f, i32, i32, i32, i32, i32, i32, i32, i32, i32,

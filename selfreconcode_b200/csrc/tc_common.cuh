@@ -11,21 +11,22 @@ namespace sr_tc {
 #define SR_TC_PLANES 2
 #endif
 constexpr int kPlanes = SR_TC_PLANES;
-constexpr int BM = 128, BN = 256, BK = 32, STAGES = kPlanes == 2 ? 3 : 2;
+// BN = the column tile of a layer launch; layers with N <= BN_NARROW run (and their weights are packed) on the
+// narrow tile instead (tile_n)
+constexpr int BM = 128, BN = 256, BN_NARROW = 64, BK = 32, STAGES = kPlanes == 2 ? 3 : 2;
 constexpr int A_PLANE = BM * BK;          // elements
-constexpr int W_PLANE = BN * BK;
 constexpr int A_STAGE = kPlanes * A_PLANE;   // 2 planes: 16 KB
-constexpr int W_STAGE = kPlanes * W_PLANE;   // 2 planes: 32 KB
-constexpr uint32_t A_STAGE_BYTES = A_STAGE * 2, W_STAGE_BYTES = W_STAGE * 2;
+constexpr uint32_t A_STAGE_BYTES = A_STAGE * 2;
+__host__ __device__ constexpr int tile_n(int N) { return N <= BN_NARROW ? BN_NARROW : BN; }
 
 // ---- tiled ("pre-swizzled") global layouts ----------------------------------------------------
 // A: [row tile mt][k chunk kc][plane p][k8 (4)][row group (16)][row (8)][elem (8)]
-// W: [col tile nt][k chunk kc][plane p][k8 (4)][row group (32)][row (8)][elem (8)]
+// W: [col tile nt][k chunk kc][plane p][k8 (4)][row group (bn / 8)][row (8)][elem (8)], bn = tile_n(N)
 __host__ __device__ inline size_t a_tile_off(long long mt, int kc, int KC, int p) {
   return (((size_t)mt * KC + kc) * kPlanes + p) * A_PLANE;
 }
-__host__ __device__ inline size_t w_tile_off(int nt, int kc, int KC, int p) {
-  return (((size_t)nt * KC + kc) * kPlanes + p) * W_PLANE;
+__host__ __device__ inline size_t w_tile_off(int bn, int nt, int kc, int KC, int p) {
+  return (((size_t)nt * KC + kc) * kPlanes + p) * (size_t)(bn * BK);
 }
 __device__ __forceinline__ int in_tile_off(int rows_per_tile, int r, int k) {
   return (k >> 3) * (rows_per_tile * 8) + (r >> 3) * 64 + (r & 7) * 8 + (k & 7);
@@ -89,8 +90,26 @@ __device__ __forceinline__ void wgmma_m64n256k16(float (&d)[128], uint64_t adesc
                  : SR_ACC128(SR_INOUT, d)
                  : "l"(adesc), "l"(bdesc), "r"(1), "n"(TA), "n"(TB));
 }
+#define SR_WGMMA_M64N64K16_BF16                                                                                    \
+  "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"                                                             \
+  "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "                                                          \
+  "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, "     \
+  "%23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n\t}\n"
+// The same for a 64-column tile: d[32], the fragment as above with i < 8.
+template <int TA, int TB, bool FIRST>
+__device__ __forceinline__ void wgmma_m64n64k16(float (&d)[32], uint64_t adesc, uint64_t bdesc) {
+  if constexpr (FIRST)
+    asm volatile(SR_WGMMA_M64N64K16_BF16
+                 : SR_ACC32(SR_OUT, d, 0)
+                 : "l"(adesc), "l"(bdesc), "r"(0), "n"(TA), "n"(TB));
+  else
+    asm volatile(SR_WGMMA_M64N64K16_BF16
+                 : SR_ACC32(SR_INOUT, d, 0)
+                 : "l"(adesc), "l"(bdesc), "r"(1), "n"(TA), "n"(TB));
+}
 #undef SR_OUT
 #undef SR_INOUT
+#undef SR_WGMMA_M64N64K16_BF16
 #undef SR_WGMMA_M64N256K16_BF16
 #undef SR_ACC128
 #undef SR_ACC32

@@ -10,7 +10,7 @@
 //
 // One launch runs one layer  C[M x N] = act(A[M x K] * W^T + b)  over all row tiles:
 //   * operands live in global memory already in the canonical (no-swizzle, K-major) shared memory layout
-//     of the wgmma descriptors -- 128-byte core matrices (8 rows x 8 bf16), tiles of 128 (or 256) rows
+//     of the wgmma descriptors -- 128-byte core matrices (8 rows x 8 bf16), tiles of 128 (or 256 / 64) rows
 //     x 32 k, the split planes of a tile contiguous -- so ONE TMA bulk copy (cp.async.bulk + mbarrier)
 //     per operand per stage lands a ready-to-use tile and no tensor map is needed.  The previous layer's
 //     epilogue writes its output directly in that layout (activations stay L2-resident between layers
@@ -19,7 +19,7 @@
 //     each, then the epilogue of those rows (bias, activation, forward-mode tangent scaling or
 //     reverse-mode act' multiply, re-split to bf16 planes, tiled store); the epilogue is specialised at
 //     compile time per (activation, rows-per-point, mode);
-//   * 3-stage shared-memory ring (48 KB per stage): the bulk copies of the next tile run under the epilogue, the
+//   * 3-stage shared-memory ring (48 KB per stage, 24 KB on the narrow column tile): the bulk copies of the next tile run under the epilogue, the
 //     MMAs do not (both consumer warpgroups are in the epilogue of the same tile; DESIGN.md section 8).
 // The FFMA engine (mlp_kernels.cu) stays the accuracy reference; tests compare both.
 #include <cstdlib>
@@ -30,11 +30,11 @@ namespace sr_tc {
 
 struct LayerArgs {
   const __nv_bfloat16* A;   // tiled activations  [MT][KC][3][128x32]
-  const __nv_bfloat16* W;   // tiled weights      [NT][KC][planes][256x32]
-  const float* bias;        // [NT*256]
+  const __nv_bfloat16* W;   // tiled weights      [NT][KC][planes][bn x 32], bn = tile_n(n_gemm)
+  const float* bias;        // [pad256(n_gemm)]
   long long M;              // valid rows
-  int MT, NT, KC;           // row tiles, col tiles, k chunks (K = 32*KC)
-  int n_gemm;               // columns the GEMM produces (<= NT*256); the MMAs always run N = 256 over zero-padded
+  int MT, NT, KC;           // row tiles, col tiles (of bn columns), k chunks (K = 32*KC)
+  int n_gemm;               // columns the GEMM produces (<= NT*bn); the MMAs always run N = bn over zero-padded
                             // weight rows, the epilogue skips the chunks past n_gemm
   int n;                    // valid output columns
   int ch;                   // rows per point: 1 (value only) or 4 (value + 3 tangents)
@@ -135,19 +135,17 @@ __device__ __forceinline__ void split3x2(float x0, float x1, uint32_t& p1, uint3
 
 struct EpiRow {
   long long mt, row;
-  int nt, row_in_tile, lane;
+  int row_in_tile, lane;
   bool row_ok, is_val;
   size_t ds_ld;
 };
 
-// One 32-column chunk of the accumulator (this thread: one row): bias / activation / tangent
-// scaling (forward) or act' multiply (reverse), then the fp32 outputs, the act' stash and the
-// re-split bf16 tile of the next layer.  `live` = the chunk holds GEMM columns (else only the
-// zero padding / skip-connection columns of the next layer's input are produced).
+// One 32-column chunk of the accumulator (this thread: one row), layer columns [c0, c0 + 32): bias / activation /
+// tangent scaling (forward) or act' multiply (reverse), then the fp32 outputs, the act' stash and the re-split bf16
+// tile of the next layer.  `live` = the chunk holds GEMM columns (else only the zero padding / skip-connection columns
+// of the next layer's input are produced).
 template <int ACT, int CH, bool MUL, bool PF = true>
-__device__ __forceinline__ void epi_chunk(const LayerArgs& a, const EpiRow& r, uint32_t (&v)[32], int chunk,
-                                          bool live) {
-  const int c0 = r.nt * BN + chunk * 32;
+__device__ __forceinline__ void epi_chunk(const LayerArgs& a, const EpiRow& r, uint32_t (&v)[32], int c0, bool live) {
   float o[32];
   if (live) {
     if constexpr (MUL) {
@@ -321,12 +319,13 @@ __device__ __forceinline__ void epi_chunk(const LayerArgs& a, const EpiRow& r, u
 // ---- the layer kernel: one layer per launch ------------------------------------------------------------------------
 // The name tc_sweep_kernel is kept: the benchmark's roofline label names it and tools/prof_train_kernels.py matches it.
 // Persistent CTAs, at most one per SM: CTA c owns the row tiles {c, c + grid, ...} and runs every n-tile of each.
-// Narrow layers (N < 256: the SDF's last layer, the input gradient of the reverse sweep) run as one N = 256 tile on
-// zero-padded weight rows.
+// The column tile is TBN = 256, or 64 for narrow layers (N <= 64: the SDF's last layer, the translator's output, the
+// input gradient of a reverse sweep): a 64-column tile streams a quarter of the weight bytes per k chunk and issues
+// n64 MMAs, where a 256-column tile would multiply zero-padded weight rows.
 //
 // Roles (3 warpgroups): warpgroup 0 = TMA producer (one thread), warpgroups 1 and 2 = rows [0, 64) and [64, 128) of
-// the 128 x 256 output tile: wgmma m64n256k16 with fp32 accumulators in registers (128 per thread), then the
-// epilogue of the same rows.  The accumulator goes through shared memory (128 columns at a time) so that each
+// the 128 x TBN output tile: wgmma m64nTBNk16 with fp32 accumulators in registers (TBN / 2 per thread), then the
+// epilogue of the same rows.  The accumulator goes through shared memory (up to 128 columns at a time) so that each
 // epilogue thread owns one row and 32 consecutive columns per chunk: the four rows of a point (value + 3 tangents)
 // sit in four consecutive lanes.
 constexpr int kConsumerWGs = 2;
@@ -334,14 +333,19 @@ constexpr int kThreads = 128 * (1 + kConsumerWGs);
 constexpr int kEpiWarps = 4 * kConsumerWGs;
 constexpr int STG_LD = 132;                 // staging row pitch (floats): conflict-free float4 row reads
 constexpr int STG_FLOATS = 64 * STG_LD;     // per consumer warpgroup: 64 rows x 128 columns
-constexpr size_t kSmem = (size_t)STAGES * (A_STAGE_BYTES + W_STAGE_BYTES) + (size_t)kConsumerWGs * STG_FLOATS * 4 + 256;
-static_assert(kSmem <= 227 * 1024, "shared memory of one H100 block");
+template <int TBN>
+constexpr uint32_t w_stage_bytes() { return (uint32_t)kPlanes * TBN * BK * 2; }   // 2 planes: 32 KB (TBN 256), 8 KB (64)
+template <int TBN>
+constexpr size_t smem_bytes() {
+  return (size_t)STAGES * (A_STAGE_BYTES + w_stage_bytes<TBN>()) + (size_t)kConsumerWGs * STG_FLOATS * 4 + 256;
+}
+static_assert(smem_bytes<BN>() <= 227 * 1024, "shared memory of one H100 block");
 
-// One k chunk of this warpgroup's 64 x 256 tile: the split-bf16 product terms, plane pairs smallest contributions
+// One k chunk of this warpgroup's 64 x TBN tile: the split-bf16 product terms, plane pairs smallest contributions
 // first -- 2 planes: (a0,w1) (a1,w0) (a0,w0); 3 planes: (a0,w2) (a2,w0) (a1,w1) (a0,w1) (a1,w0) (a0,w0).
 // abase = this warpgroup's first row group of the A stage, wbase = the W stage.
-template <bool FIRST>
-__device__ __forceinline__ void mma_chunk(float (&acc)[128], uint32_t abase, uint32_t wbase) {
+template <int TBN, bool FIRST>
+__device__ __forceinline__ void mma_chunk(float (&acc)[TBN / 2], uint32_t abase, uint32_t wbase) {
   constexpr int kTerms = kPlanes == 2 ? 3 : 6;
   const int pa[6] = {0, 1, 0, 2, 1, 0}, pw[6] = {1, 0, 0, 0, 1, 0};
   const int pa3[6] = {0, 2, 1, 0, 1, 0}, pw3[6] = {2, 0, 1, 1, 0, 0};
@@ -352,16 +356,26 @@ __device__ __forceinline__ void mma_chunk(float (&acc)[128], uint32_t abase, uin
       // K = 16 per MMA = two 8-wide core matrices: advance two LBO steps per jj
       const int qa = kPlanes == 2 ? pa[q] : pa3[q], qw = kPlanes == 2 ? pw[q] : pw3[q];
       const uint64_t ad = make_desc(abase + qa * (A_PLANE * 2) + jj * 2 * (BM * 16), BM * 16, 128);
-      const uint64_t bd = make_desc(wbase + qw * (W_PLANE * 2) + jj * 2 * (BN * 16), BN * 16, 128);
-      if (FIRST && q == 0 && jj == 0) wgmma_m64n256k16<0, 0, true>(acc, ad, bd);
-      else wgmma_m64n256k16<0, 0, false>(acc, ad, bd);
+      const uint64_t bd = make_desc(wbase + qw * (TBN * BK * 2) + jj * 2 * (TBN * 16), TBN * 16, 128);
+      const bool first = FIRST && q == 0 && jj == 0;
+      if constexpr (TBN == BN) {
+        if (first) wgmma_m64n256k16<0, 0, true>(acc, ad, bd);
+        else wgmma_m64n256k16<0, 0, false>(acc, ad, bd);
+      } else {
+        static_assert(TBN == BN_NARROW, "column tile");
+        if (first) wgmma_m64n64k16<0, 0, true>(acc, ad, bd);
+        else wgmma_m64n64k16<0, 0, false>(acc, ad, bd);
+      }
     }
   }
 }
 
-// <ACT, CH, MUL>: the layer's activation (a reverse launch: the PREVIOUS layer's), rows per point, reverse mode
-template <int ACT, int CH, bool MUL>
+// <ACT, CH, MUL, TBN>: the layer's activation (a reverse launch: the PREVIOUS layer's), rows per point, reverse mode,
+// column tile
+template <int ACT, int CH, bool MUL, int TBN>
 __global__ void __launch_bounds__(kThreads, 1) tc_sweep_kernel(const __grid_constant__ LayerArgs a) {
+  constexpr uint32_t W_STAGE_BYTES = w_stage_bytes<TBN>();
+  constexpr int W_STAGE = W_STAGE_BYTES / 2;   // elements
   extern __shared__ __align__(1024) unsigned char smem[];
   __nv_bfloat16* sA = reinterpret_cast<__nv_bfloat16*>(smem);
   __nv_bfloat16* sW = reinterpret_cast<__nv_bfloat16*>(smem + (size_t)STAGES * A_STAGE_BYTES);
@@ -400,7 +414,7 @@ __global__ void __launch_bounds__(kThreads, 1) tc_sweep_kernel(const __grid_cons
           for (int kc = 0; kc < a.KC; ++kc) {
             sr_mbar_wait(&empty[slot], phase ^ 1u);
             sr_mbar_arrive_expect_tx(&full[slot], A_STAGE_BYTES + W_STAGE_BYTES);
-            sr_bulk_g2s(sW + (size_t)slot * W_STAGE, a.W + w_tile_off(nt, kc, a.KC, 0), W_STAGE_BYTES, &full[slot]);
+            sr_bulk_g2s(sW + (size_t)slot * W_STAGE, a.W + w_tile_off(TBN, nt, kc, a.KC, 0), W_STAGE_BYTES, &full[slot]);
             sr_bulk_g2s(sA + (size_t)slot * A_STAGE, a.A + a_tile_off(mt, kc, a.KC, 0), A_STAGE_BYTES, &full[slot]);
             if (++slot == STAGES) { slot = 0; phase ^= 1u; }
           }
@@ -413,14 +427,14 @@ __global__ void __launch_bounds__(kThreads, 1) tc_sweep_kernel(const __grid_cons
     const int cw = wg - 1;                  // rows [64 cw, 64 cw + 64) of the row tile
     const int wq = warp & 3;                // warp in the warpgroup
     float* st = stg + cw * STG_FLOATS;
-    float acc[128];
+    float acc[TBN / 2];
     EpiRow r;
     r.row_in_tile = cw * 64 + (wq & 1) * 32 + lane;
     r.lane = lane;
     r.is_val = (CH == 1) || ((lane & 3) == 0);
-    // act' stash pitch: a forward launch writes pad256(N); a reverse launch reads the previous layer's stash, whose
-    // width is this launch's n (N = n + d_in for a skip layer, which may cross a multiple of 256)
-    r.ds_ld = MUL ? (size_t)((a.n + BN - 1) / BN) * BN : (size_t)a.NT * BN;
+    // act' stash pitch (either column tile): a forward launch writes pad256(N); a reverse launch reads the previous
+    // layer's stash, whose width is this launch's n (N = n + d_in for a skip layer, which may cross a multiple of 256)
+    r.ds_ld = (size_t)(((MUL ? a.n : a.n_gemm) + BN - 1) / BN) * BN;
     int slot = 0;
     uint32_t phase = 0;
     for (int j = 0; j < J; ++j) {
@@ -428,20 +442,19 @@ __global__ void __launch_bounds__(kThreads, 1) tc_sweep_kernel(const __grid_cons
       r.row = r.mt * BM + r.row_in_tile;
       r.row_ok = r.row < Mrows;
       for (int nt = 0; nt < a.NT; ++nt) {
-        r.nt = nt;
         // the first k chunk overwrites the accumulator (it is dead from here back to the previous epilogue)
         sr_mbar_wait(&full[slot], phase);
         wgmma_fence();
-        mma_chunk<true>(acc, sr_smem_u32(sA + (size_t)slot * A_STAGE) + cw * 8 * 128,
-                        sr_smem_u32(sW + (size_t)slot * W_STAGE));
+        mma_chunk<TBN, true>(acc, sr_smem_u32(sA + (size_t)slot * A_STAGE) + cw * 8 * 128,
+                             sr_smem_u32(sW + (size_t)slot * W_STAGE));
         wgmma_commit();
         int prev = slot;
         if (++slot == STAGES) { slot = 0; phase ^= 1u; }
         for (int kc = 1; kc < a.KC; ++kc) {
           sr_mbar_wait(&full[slot], phase);
           wgmma_fence();
-          mma_chunk<false>(acc, sr_smem_u32(sA + (size_t)slot * A_STAGE) + cw * 8 * 128,
-                           sr_smem_u32(sW + (size_t)slot * W_STAGE));
+          mma_chunk<TBN, false>(acc, sr_smem_u32(sA + (size_t)slot * A_STAGE) + cw * 8 * 128,
+                                sr_smem_u32(sW + (size_t)slot * W_STAGE));
           wgmma_commit();
           wgmma_wait<1>();   // the previous stage's MMAs are complete: release it
           if (lane == 0) sr_mbar_arrive(&empty[prev]);
@@ -450,22 +463,23 @@ __global__ void __launch_bounds__(kThreads, 1) tc_sweep_kernel(const __grid_cons
         }
         wgmma_wait<0>();
         if (lane == 0) sr_mbar_arrive(&empty[prev]);
-        // epilogue: 128 accumulator columns per pass through the staging buffer; warp wq handles rows
-        // 32 (wq & 1) + lane and the 64 columns 64 (wq >> 1) of each pass (two 32-column chunks)
+        // epilogue: PASS accumulator columns per pass through the staging buffer; warp wq handles rows
+        // 32 (wq & 1) + lane and the PASS / 2 columns (PASS / 2) (wq >> 1) of each pass (PASS / 64 32-column chunks)
+        constexpr int PASS = TBN < 128 ? TBN : 128, FRAGS = PASS / 8, WCH = PASS / 64;
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
+        for (int h = 0; h < TBN / PASS; ++h) {
           const int fr = 16 * wq + (lane >> 2), fc = 2 * (lane & 3);
 #pragma unroll
-          for (int i = 0; i < 16; ++i) {
+          for (int i = 0; i < FRAGS; ++i) {
             *reinterpret_cast<float2*>(st + fr * STG_LD + 8 * i + fc) =
-                make_float2(acc[4 * (16 * h + i)], acc[4 * (16 * h + i) + 1]);
+                make_float2(acc[4 * (FRAGS * h + i)], acc[4 * (FRAGS * h + i) + 1]);
             *reinterpret_cast<float2*>(st + (fr + 8) * STG_LD + 8 * i + fc) =
-                make_float2(acc[4 * (16 * h + i) + 2], acc[4 * (16 * h + i) + 3]);
+                make_float2(acc[4 * (FRAGS * h + i) + 2], acc[4 * (FRAGS * h + i) + 3]);
           }
           warpgroup_sync(1 + cw);
-          const float* srow = st + ((wq & 1) * 32 + lane) * STG_LD + (wq >> 1) * 64;
-          for (int i = 0; i < 2; ++i) {
-            const int chunk = 4 * h + 2 * (wq >> 1) + i;
+          const float* srow = st + ((wq & 1) * 32 + lane) * STG_LD + (wq >> 1) * (PASS / 2);
+          for (int i = 0; i < WCH; ++i) {
+            const int c0 = nt * TBN + h * PASS + (wq >> 1) * (PASS / 2) + 32 * i;
             uint32_t v[32];
 #pragma unroll
             for (int j4 = 0; j4 < 8; ++j4) {
@@ -473,7 +487,7 @@ __global__ void __launch_bounds__(kThreads, 1) tc_sweep_kernel(const __grid_cons
               v[4 * j4] = __float_as_uint(t.x); v[4 * j4 + 1] = __float_as_uint(t.y);
               v[4 * j4 + 2] = __float_as_uint(t.z); v[4 * j4 + 3] = __float_as_uint(t.w);
             }
-            epi_chunk<ACT, CH, MUL>(a, r, v, chunk, nt * BN + chunk * 32 < a.n_gemm);
+            epi_chunk<ACT, CH, MUL>(a, r, v, c0, c0 < a.n_gemm);
           }
           warpgroup_sync(1 + cw);
         }
@@ -553,17 +567,18 @@ __global__ void pack_skip_tail_kernel(const float* __restrict__ skip_src, int sk
   }
 }
 
-// effective weights, fp32 row-major [N][K] (ld) -> tiled split-bf16 [NT][KC][planes][256x32]
+// effective weights, fp32 row-major [N][K] (ld) -> tiled split-bf16 [NT][KC][planes][bn x 32], bn = tile_n(N)
 __global__ void pack_weights_kernel(const float* __restrict__ w, int N, int K, int ld,
                                     __nv_bfloat16* __restrict__ dst, int NT, int KC) {
-  const long long total = (long long)NT * BN * KC * 4;
+  const int bn = tile_n(N);
+  const long long total = (long long)NT * bn * KC * 4;
   for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
        idx += (long long)gridDim.x * blockDim.x) {
-    const int r = (int)(idx % BN);
-    const long long rest = idx / BN;
+    const int r = (int)(idx % bn);
+    const long long rest = idx / bn;
     const int g = (int)(rest % (KC * 4));
     const int nt = (int)(rest / (KC * 4));
-    const int n = nt * BN + r;
+    const int n = nt * bn + r;
     const int kc = g >> 2, k8 = g & 3;
     __align__(16) __nv_bfloat16 p1[8], p2[8], p3[8];
 #pragma unroll
@@ -572,11 +587,11 @@ __global__ void pack_weights_kernel(const float* __restrict__ w, int N, int K, i
       const float x = (n < N && k < K) ? w[(size_t)n * ld + k] : 0.f;
       split3(x, p1[e], p2[e], p3[e]);
     }
-    const size_t off = (size_t)k8 * (BN * 8) + (size_t)(r >> 3) * 64 + (r & 7) * 8;
-    *reinterpret_cast<uint4*>(dst + w_tile_off(nt, kc, KC, 0) + off) = *reinterpret_cast<uint4*>(p1);
-    *reinterpret_cast<uint4*>(dst + w_tile_off(nt, kc, KC, 1) + off) = *reinterpret_cast<uint4*>(p2);
+    const size_t off = (size_t)k8 * (bn * 8) + (size_t)(r >> 3) * 64 + (r & 7) * 8;
+    *reinterpret_cast<uint4*>(dst + w_tile_off(bn, nt, kc, KC, 0) + off) = *reinterpret_cast<uint4*>(p1);
+    *reinterpret_cast<uint4*>(dst + w_tile_off(bn, nt, kc, KC, 1) + off) = *reinterpret_cast<uint4*>(p2);
     if constexpr (kPlanes == 3)
-      *reinterpret_cast<uint4*>(dst + w_tile_off(nt, kc, KC, kPlanes - 1) + off) = *reinterpret_cast<uint4*>(p3);
+      *reinterpret_cast<uint4*>(dst + w_tile_off(bn, nt, kc, KC, kPlanes - 1) + off) = *reinterpret_cast<uint4*>(p3);
   }
 }
 
@@ -634,18 +649,20 @@ __global__ void embed_kernel(const __grid_constant__ EmbedArgs a) {
 }
 
 // Backward of embed_kernel w.r.t. the points: gx [P*ch][ld] cotangent rows -> gp [P][3].  Value row: d PE / d p; tangent
-// rows (ch = 4): the tangent entries themselves depend on p (second derivative of the encoding).  One thread per point.
+// rows (ch = 4): the tangent entries themselves depend on p (second derivative of the encoding).  gk (ch = 1, or null):
+// a second cotangent of the same input, [P][gk_ld] -- a skip layer's part of the reverse sweep.  One thread per point.
 __global__ void embed_bwd_kernel(const float* __restrict__ pts, long long P, int multires, const float* __restrict__ gx,
-                                 int ld, int ch, float* __restrict__ gp, float pw0, float pw1, float pw2, float pw3,
-                                 float pw4, float pw5, float pw6, float pw7) {
+                                 int ld, int ch, const float* __restrict__ gk, int gk_ld, float* __restrict__ gp,
+                                 float pw0, float pw1, float pw2, float pw3, float pw4, float pw5, float pw6, float pw7) {
   const float pw[8] = {pw0, pw1, pw2, pw3, pw4, pw5, pw6, pw7};
   for (long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x; p < P; p += (long long)gridDim.x * blockDim.x) {
     const float* gv = gx + (size_t)p * ch * ld;
+    const float* gs = gk != nullptr ? gk + (size_t)p * gk_ld : nullptr;
     float out[3];
 #pragma unroll
     for (int j = 0; j < 3; ++j) {
       const float x = pts[p * 3 + j];
-      float acc = gv[j];
+      float acc = gv[j] + (gs ? gs[j] : 0.f);
       const float* gt = ch == 4 ? gv + (size_t)(1 + j) * ld : nullptr;   // tangent row d/dp_j: only column j is non-zero
       float freq = 1.0f;
       for (int b = 0; b < multires; ++b, freq *= 2.0f) {
@@ -653,7 +670,8 @@ __global__ void embed_bwd_kernel(const float* __restrict__ pts, long long P, int
         sincosf(x * freq, &sn, &cs);
         const float w = pw[b] * freq;
         const int ks = 3 + 6 * b + j, kc = ks + 3;
-        acc += w * (cs * gv[ks] - sn * gv[kc]);
+        const float gsn = gv[ks] + (gs ? gs[ks] : 0.f), gcs = gv[kc] + (gs ? gs[kc] : 0.f);
+        acc += w * (cs * gsn - sn * gcs);
         if (gt) acc -= w * freq * (sn * gt[ks] + cs * gt[kc]);
       }
       out[j] = acc;
@@ -667,14 +685,14 @@ __global__ void embed_bwd_kernel(const float* __restrict__ pts, long long P, int
 extern "C" {
 
 int sr_tc_embed_backward(const float* pts, int64_t P, int multires, const float* pe_w, int ch, const float* gx, int ld,
-                         float* gp, cudaStream_t s) {
+                         const float* gk, int gk_ld, float* gp, cudaStream_t s) {
   if (!pts || !gx || !gp || !pe_w || P <= 0 || (ch != 1 && ch != 4) || multires < 0 || multires > 8 ||
-      ld < 3 + 6 * multires)
+      ld < 3 + 6 * multires || (gk && (ch != 1 || gk_ld < 3 + 6 * multires)))
     return SR_EINVAL;
   float w[8];
   for (int i = 0; i < 8; ++i) w[i] = i < multires ? pe_w[i] : 0.f;
-  sr_tc::embed_bwd_kernel<<<sr_grid_for(P, 256, 8), 256, 0, s>>>(pts, P, multires, gx, ld, ch, gp, w[0], w[1], w[2], w[3],
-                                                                  w[4], w[5], w[6], w[7]);
+  sr_tc::embed_bwd_kernel<<<sr_grid_for(P, 256, 8), 256, 0, s>>>(pts, P, multires, gx, ld, ch, gk, gk_ld, gp, w[0], w[1],
+                                                                  w[2], w[3], w[4], w[5], w[6], w[7]);
   return sr_launch_status();
 }
 
@@ -698,8 +716,8 @@ int64_t sr_tc_act_bytes(int64_t M, int K) {
   return MT * KC * sr_tc::kPlanes * sr_tc::A_PLANE * 2;
 }
 int64_t sr_tc_weight_bytes(int N, int K) {
-  const int64_t NT = (N + sr_tc::BN - 1) / sr_tc::BN, KC = (K + 31) / 32;
-  return NT * KC * sr_tc::kPlanes * sr_tc::W_PLANE * 2;
+  const int64_t bn = sr_tc::tile_n(N), NT = (N + bn - 1) / bn, KC = (K + 31) / 32;
+  return NT * KC * sr_tc::kPlanes * bn * sr_tc::BK * 2;
 }
 
 int sr_tc_pack_rows(const float* src, int64_t M, int K, int ld, void* dst, const int32_t* m_dev,
@@ -714,8 +732,8 @@ int sr_tc_pack_rows(const float* src, int64_t M, int K, int ld, void* dst, const
 
 int sr_tc_pack_weights(const float* w, int N, int K, int ld, void* dst, cudaStream_t s) {
   if (!w || !dst || N <= 0 || K <= 0 || ld < K) return SR_EINVAL;
-  const int NT = (N + sr_tc::BN - 1) / sr_tc::BN, KC = (K + 31) / 32;
-  const long long total = (long long)NT * sr_tc::BN * KC * 4;
+  const int bn = sr_tc::tile_n(N), NT = (N + bn - 1) / bn, KC = (K + 31) / 32;
+  const long long total = (long long)NT * bn * KC * 4;
   sr_tc::pack_weights_kernel<<<sr_grid_for(total, 256, 8), 256, 0, s>>>(w, N, K, ld, (__nv_bfloat16*)dst, NT, KC);
   return sr_launch_status();
 }
@@ -735,8 +753,9 @@ int sr_tc_linear(const void* A, const void* W, const float* bias, int64_t M, int
                 : (act < SR_ACT_NONE || act > SR_ACT_TANH))
     return SR_EINVAL;
   LayerArgs a;
+  const int bn = tile_n(N);   // the column tile W was packed with (sr_tc_pack_weights of the same N)
   a.A = (const __nv_bfloat16*)A; a.W = (const __nv_bfloat16*)W; a.bias = bias; a.M = M;
-  a.MT = (int)((M + BM - 1) / BM); a.NT = (N + BN - 1) / BN; a.KC = (K + 31) / 32;
+  a.MT = (int)((M + BM - 1) / BM); a.NT = (N + bn - 1) / bn; a.KC = (K + 31) / 32;
   a.n_gemm = N; a.n = n_valid; a.ch = ch;
   a.A_next = (__nv_bfloat16*)A_next; a.KCn = A_next ? (K_next + 31) / 32 : 0;
   a.scale = scale; a.skip_src = skip_src; a.skip_n = skip_n; a.skip_ld = skip_ld;
@@ -746,7 +765,9 @@ int sr_tc_linear(const void* A, const void* W, const float* bias, int64_t M, int
 
   using Kern = void (*)(const LayerArgs);
   Kern kern = nullptr;
-#define SR_SW(ACT_, CH_, MUL_) kern = (Kern)tc_sweep_kernel<ACT_, CH_, MUL_>
+  const bool narrow = bn == BN_NARROW;
+#define SR_SW(ACT_, CH_, MUL_)                                                                    \
+  kern = narrow ? (Kern)tc_sweep_kernel<ACT_, CH_, MUL_, BN_NARROW> : (Kern)tc_sweep_kernel<ACT_, CH_, MUL_, BN>
   const int key = (ch == 4 ? 10 : 0) + (mul_tiles ? 5 + mul_act : act);
   switch (key) {
     case 0: SR_SW(SR_ACT_NONE, 1, false); break;
@@ -767,18 +788,19 @@ int sr_tc_linear(const void* A, const void* W, const float* bias, int64_t M, int
 #undef SR_SW
   if (!kern) return SR_EINVAL;
   // cudaFuncSetAttribute is per device: one flag per device ordinal (a process may drive several GPUs)
-  static bool attr_set_dev[64][20] = {};
+  static bool attr_set_dev[64][2][20] = {};
   int cur_dev = 0;
   cudaGetDevice(&cur_dev);
-  bool& attr_set = attr_set_dev[cur_dev & 63][key];
+  bool& attr_set = attr_set_dev[cur_dev & 63][narrow][key];
+  const size_t smem = narrow ? smem_bytes<BN_NARROW>() : smem_bytes<BN>();
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmem);
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return (int)e;
     attr_set = true;
   }
   const int grid = a.MT < SR_NUM_SMS ? a.MT : SR_NUM_SMS;
-  kern<<<grid, kThreads, kSmem, s>>>(a);
-  const int kc0 = a.NT * (BN / 32);   // first next-layer chunk the epilogue does not produce
+  kern<<<grid, kThreads, smem, s>>>(a);
+  const int kc0 = a.NT * (bn / 32);   // first next-layer chunk the epilogue does not produce
   if (a.A_next != nullptr && a.KCn > kc0) {
     const int rc = sr_launch_status();
     if (rc) return rc;

@@ -179,8 +179,7 @@ struct ShadePtArgs {
   const float* pts;
   const float* rays;
   const long long* batch_inds;
-  const float* sdf4;   // [P*4][ld_s]: col 0 of rows 4p+1..4p+3 = grad f
-  int ld_s;
+  const float* grad;   // [P][3] grad f
   const float* off4;   // [P*4][3] translator offset (row 4p) and its tangents (rows 4p+1..3), or null
   sr_lbs_params lbs;
   int has_lbs;
@@ -222,7 +221,7 @@ __global__ void __launch_bounds__(256) shade_point_kernel(const __grid_constant_
       for (int r = 0; r < 3; ++r)
 #pragma unroll
         for (int c = 0; c < 3; ++c) m[3 * r + c] = Mm[3 * r] * Q[c] + Mm[3 * r + 1] * Q[3 + c] + Mm[3 * r + 2] * Q[6 + c];
-      const float gx = a.sdf4[(i * 4 + 1) * a.ld_s], gy = a.sdf4[(i * 4 + 2) * a.ld_s], gz = a.sdf4[(i * 4 + 3) * a.ld_s];
+      const float gx = a.grad[i * 3], gy = a.grad[i * 3 + 1], gz = a.grad[i * 3 + 2];
       const float gn = sqrtf(gx * gx + gy * gy + gz * gz);
       a.normals[i * 3] = gx / gn; a.normals[i * 3 + 1] = gy / gn; a.normals[i * 3 + 2] = gz / gn;
       const float c00 = m[4] * m[8] - m[5] * m[7], c01 = -m[3] * m[8] + m[5] * m[6], c02 = m[3] * m[7] - m[4] * m[6];
@@ -288,12 +287,12 @@ __global__ void render_embed_kernel(const __grid_constant__ RenderEmbedArgs a) {
 extern "C" {
 
 int sr_tc_shade_point(int64_t P, const float* pts, const float* rays, const int64_t* batch_inds,
-                      const float* sdf4, int ld_s, const float* off4, const sr_lbs_params* lbs,
+                      const float* grad, const float* off4, const sr_lbs_params* lbs,
                       float* normals, float* crays, float* dpos, uint8_t* inv_ok, cudaStream_t s) {
-  if (P <= 0 || !pts || !rays || !sdf4 || !normals || !crays) return SR_EINVAL;
+  if (P <= 0 || !pts || !rays || !grad || !normals || !crays) return SR_EINVAL;
   ShadePtArgs a;
-  a.P = P; a.pts = pts; a.rays = rays; a.batch_inds = (const long long*)batch_inds; a.sdf4 = sdf4;
-  a.ld_s = ld_s; a.off4 = off4; a.has_lbs = lbs ? 1 : 0;
+  a.P = P; a.pts = pts; a.rays = rays; a.batch_inds = (const long long*)batch_inds; a.grad = grad;
+  a.off4 = off4; a.has_lbs = lbs ? 1 : 0;
   if (lbs) a.lbs = *lbs;
   a.normals = normals; a.crays = crays; a.dpos = dpos; a.inv_ok = inv_ok;
   shade_point_kernel<<<sr_grid_for(P * 32, 256, 8), 256, 0, s>>>(a);

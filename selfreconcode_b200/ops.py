@@ -436,7 +436,11 @@ class FusedMLP:
 
     def truncated_last(self, n_out):
         """A view of the same network whose last layer only produces the first n_out outputs
-        (e.g. the SDF value without the 256-d feature): same buffers, narrower npad."""
+        (e.g. the SDF value without the 256-d feature): same buffers, narrower npad.  One view per n_out: later calls
+        return it again, so its copies and tensor-core packs exist (and are refreshed on refold) once."""
+        for c in self._children:
+            if c.desc.layer[c.desc.n_layers - 1].n == n_out:
+                return c
         t = FusedMLP(self.d_in, self.multires, self.device)
         C.memmove(C.byref(t.desc), C.byref(self.desc), C.sizeof(MlpDesc))
         last = t.desc.layer[t.desc.n_layers - 1]
@@ -860,6 +864,7 @@ class TcNet:
             self.layers.append(dict(W=W, Wb=Wb, bias=torch.zeros((_pad(n, 256),), dtype=torch.float32, device=dev),
                                     n=n, k=k, act=ly.act, skip=bool(ly.skip), _e=e,
                                     zero_bias=torch.zeros((_pad(k, 256),), dtype=torch.float32, device=dev)))
+        self._wb_head = {}     # n_keep -> pack of the first n_keep rows of the input layer's W^T (wb_head)
         # the same packs as sr_tc_mlp_forward's layer array (repack() keeps the buffers, so the pointers stay valid)
         self.c_layers = (_lib.TcLayer * len(self.layers))()
         for c, L in zip(self.c_layers, self.layers):
@@ -878,6 +883,28 @@ class TcNet:
                 check(lib.sr_tc_pack_weights(_p(e["wt"]), k, n, e["wt"].shape[1], _p(L["Wb"]), _stream()),
                       "tc_pack_weights")
                 L["bias"][:n].copy_(e["bias"][:n])
+            for n_keep, buf in self._wb_head.items():
+                self._pack_head(n_keep, buf)
+
+    def _pack_head(self, n_keep, buf):
+        L = self.layers[0]
+        e = L["_e"]
+        check(_lib.load().sr_tc_pack_weights(_p(e["wt"]), n_keep, L["n"], e["wt"].shape[1], _p(buf), _stream()),
+              "tc_pack_weights")
+
+    def wb_head(self, n_keep):
+        """Reverse-sweep operand of the input layer restricted to its first n_keep inputs (a narrow launch when
+        n_keep <= 64), for sweeps that need only those columns of the input gradient: the tracer's translator keeps the
+        positional-encoding part, not the latent code's.  Packed on first use, refreshed by repack()."""
+        buf = self._wb_head.get(n_keep)
+        if buf is None:
+            lib = _lib.load()
+            buf = torch.empty((lib.sr_tc_weight_bytes(n_keep, self.layers[0]["n"]),), dtype=torch.uint8,
+                              device=self.fused.device)
+            with torch.cuda.device(self.fused.device):
+                self._pack_head(n_keep, buf)
+            self._wb_head[n_keep] = buf
+        return buf
 
 
 def tc_net(fused):
@@ -987,7 +1014,8 @@ def _tc_backward_sweep(lib, tcn, cot, bufs, acts, P, m_dev, g_out, g_skip, n_kee
                                    tcn.layers[l - 1]["act"], scale, _p(m_dev), _stream()), "tc_linear")
             cur, nxt, K = nxt, cur, Kn
         else:
-            check(lib.sr_tc_linear(_p(cur), _p(ly["Wb"]), _p(ly["zero_bias"]), P, ly["k"], K, ly["k"], 0, 1, None, 0,
+            Wb, N = (tcn.wb_head(n_keep), n_keep) if n_keep < ly["k"] else (ly["Wb"], ly["k"])
+            check(lib.sr_tc_linear(_p(cur), _p(Wb), _p(ly["zero_bias"]), P, N, K, N, 0, 1, None, 0,
                                    scale, None, 0, 0, _p(g_out), g_out.shape[1], 0, n_keep, None, None, 0, 0, 1.0,
                                    _p(m_dev), _stream()), "tc_linear")
 
@@ -1192,9 +1220,66 @@ def _side_stream(dev):
     return st
 
 
+class _TcShadeBuffers:
+    """Work buffers of the SDF's reverse-mode gradient in shade_and_render_tc for up to `cap` points (the kept
+    activation tiles alone take ~0.9 GB at 50 000 points)."""
+
+    def __init__(self, dev, cap, sdf_full):
+        lib = _lib.load()
+        d = sdf_full.desc
+        f32 = lambda *shape: torch.empty(shape, dtype=torch.float32, device=dev)   # noqa: E731
+        u8 = lambda n: torch.empty((n,), dtype=torch.uint8, device=dev)           # noqa: E731
+        self.cap = cap
+        self.ld = _pad(d.d_in, 32)
+        self.emb = f32(cap, self.ld)
+        self.A_in = u8(lib.sr_tc_act_bytes(cap, self.ld))
+        self.acts = [u8(lib.sr_tc_act_bytes(cap, _pad(d.layer[i + 1].k, 32))) for i in range(d.n_layers - 1)]
+        self.out = f32(cap, d.layer[d.n_layers - 1].n)          # f + features
+        widest = max([32] + [_pad(d.layer[l].n, 32) for l in range(d.n_layers - 1)])
+        self.A = [u8(lib.sr_tc_act_bytes(cap, widest)) for _ in range(2)]
+        self.cot = torch.zeros((cap, 32), dtype=torch.float32, device=dev)
+        self.cot[:, 0] = 1.0                                     # d f / d f: the reverse sweep's seed
+        self.g_out = f32(cap, self.ld)
+        self.g_skip = f32(cap, self.ld)
+        self.grad = f32(cap, 3)
+
+
+# one buffer set per (device, SDF widths), grown (by at least a quarter, in steps of 4096 points) when a call brings
+# more points than it holds: a point count that changes from frame to frame keeps hitting it
+_tc_shade_bufs = {}
+
+
+def _sdf_grad_tc(lib, sdf_full, pts, P):
+    """SDF value + features and grad f in reverse mode: one value-only forward sweep keeping its activation tiles, one
+    reverse sweep from a cotangent of 1 on f (the value-only view's layers: the last one is 1 wide), then the chain
+    through the positional encoding.  Returns views of the cached buffers: out [P, 1 + nfeat], grad [P, 3] and the
+    encoding's cotangent without the skip layer's part, g_out [P, pad32(d_in)]."""
+    dev = pts.device
+    d = sdf_full.desc
+    key = (dev.index, tuple(d.layer[i].n for i in range(d.n_layers)), d.d_in)
+    B = _tc_shade_bufs.get(key)
+    if B is None or B.cap < P:
+        cap = _pad(max(P, B.cap + B.cap // 4 if B is not None else 0), 4096)
+        _tc_shade_bufs.pop(key, None)
+        B = None                                         # drop the smaller set before allocating its successor
+        B = _tc_shade_bufs[key] = _TcShadeBuffers(dev, cap, sdf_full)
+    ts, tv = tc_net(sdf_full), tc_net(sdf_full.truncated_last(1))
+    pw = (C.c_float * 16)(*[d.pe_w[i] for i in range(16)])
+    emb, out, grad, g_out = B.emb[:P], B.out[:P], B.grad[:P], B.g_out[:P]
+    check(lib.sr_tc_embed(_p(pts), P, d.multires, pw, 1, None, None, 0, 0, _p(emb), B.ld, None, None, _stream()),
+          "tc_embed")
+    _tc_mlp(lib, ts, emb, 1, out, B.A_in, B.acts)
+    _tc_backward_sweep(lib, tv, B.cot, B.A, B.acts, P, None, g_out, B.g_skip, d.d_in)
+    has_skip = any(l["skip"] for l in ts.layers)
+    check(lib.sr_tc_embed_backward(_p(pts), P, d.multires, pw, 1, _p(g_out), B.ld, _p(B.g_skip) if has_skip else None,
+                                   B.ld, _p(grad), _stream()), "tc_embed_backward")
+    return out, grad, g_out
+
+
 def shade_and_render_tc(sdf_full, def_net, lbs, render_net, pts, rays, batch_inds, conds, nfeat=256):
-    """Shading of the infer path on the tensor-core engine: SDF and translator sweeps with forward
-    tangents (4 rows per point), pointwise geometry, then the rendering network.
+    """Shading of the infer path on the tensor-core engine: grad f of the SDF in reverse mode (one value-only forward
+    sweep + one reverse sweep), the translator's sweep with forward tangents (4 rows per point: its 3x3 Jacobian),
+    pointwise geometry, then the rendering network.
     Returns (normals, cardinal rays, rgb, D(p), inverse-ok mask)."""
     _need_cuda(pts, rays)
     dev = pts.device
@@ -1211,23 +1296,23 @@ def shade_and_render_tc(sdf_full, def_net, lbs, render_net, pts, rays, batch_ind
             side.wait_stream(main)
             with torch.cuda.stream(side):
                 o4 = tc_mlp_forward(def_net, pts, ch=4, conds=conds, batch_inds=bi)
-            s4 = tc_mlp_forward(sdf_full, pts, ch=4)                  # [4P, 1+nfeat]
+            f_feat, grad, _ = _sdf_grad_tc(lib, sdf_full, pts, P)
             main.wait_stream(side)
             o4.record_stream(main)
         else:
-            s4 = tc_mlp_forward(sdf_full, pts, ch=4)
+            f_feat, grad, _ = _sdf_grad_tc(lib, sdf_full, pts, P)
             o4 = tc_mlp_forward(def_net, pts, ch=4, conds=conds, batch_inds=bi) if def_net is not None else None
         normals = torch.empty((P, 3), dtype=torch.float32, device=dev)
         crays = torch.empty((P, 3), dtype=torch.float32, device=dev)
         dpos = torch.empty((P, 3), dtype=torch.float32, device=dev)
         ok = torch.empty((P,), dtype=torch.bool, device=dev)
-        check(lib.sr_tc_shade_point(P, _p(pts), _p(rays), _p(bi), _p(s4), s4.shape[1], _p(o4), _lbs_ref(lbs),
+        check(lib.sr_tc_shade_point(P, _p(pts), _p(rays), _p(bi), _p(grad), _p(o4), _lbs_ref(lbs),
                                     _p(normals), _p(crays), _p(dpos), _p(ok), _stream()), "tc_shade_point")
         rd = render_net.desc
         ld = _pad(rd.d_in, 32)
         emb = torch.empty((P, ld), dtype=torch.float32, device=dev)
         pw = (C.c_float * 16)(*[rd.pe_w[i] for i in range(16)])
-        check(lib.sr_tc_render_embed(P, _p(pts), _p(crays), _p(normals), _p(s4), s4.shape[1], 1, nfeat, 4,
+        check(lib.sr_tc_render_embed(P, _p(pts), _p(crays), _p(normals), _p(f_feat), f_feat.shape[1], 1, nfeat, 1,
                                      rd.multires, pw, _p(emb), ld, _stream()), "tc_render_embed")
         rn = tc_net(render_net)
         rgb = torch.empty((P, rn.layers[-1]["n"]), dtype=torch.float32, device=dev)

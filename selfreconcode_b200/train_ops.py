@@ -262,8 +262,8 @@ class EmbedRowsFunction(torch.autograd.Function):
             gp = torch.empty((P, 3), dtype=torch.float32, device=pts.device)
             pw = (C.c_float * 16)(*[pe_w[i] if i < multires else 0.0 for i in range(16)])
             with torch.cuda.device(pts.device):
-                check(lib.sr_tc_embed_backward(_p(pts), P, multires, pw, ch, _p(gx), width, _p(gp), _stream()),
-                      "tc_embed_backward")
+                check(lib.sr_tc_embed_backward(_p(pts), P, multires, pw, ch, _p(gx), width, None, 0, _p(gp),
+                                               _stream()), "tc_embed_backward")
         if E and ctx.needs_input_grad[1]:
             pe = 3 + 6 * multires
             ge = gx.view(P, ch, width)[:, 0, pe:pe + E]
