@@ -334,6 +334,32 @@ int sr_shade_phong(const float* verts, const float* normals, const float* colors
                    const float* cam_pos, const float* light_pos, const sr_phong_params* params, float* out,
                    cudaStream_t s);
 
+/* Soft point-cloud silhouette of the template (model/network.py:495-505: pytorch3d 0.4.0 PointsRasterizer with
+ * points_per_pixel = K and radius r in NDC, then AlphaCompositor(background_color=None), all features 1), forward and
+ * backward.  pts_screen [N,V,3] = (col, row, view-space Z) per frame, pixel centres at integers.  Point p covers pixel
+ * (i, j) iff Z >= 0 and d2 = (2/W)^2 (col-j)^2 + (2/H)^2 (row-i)^2 < r^2; each pixel keeps its K covering points of
+ * smallest (Z, index) and composites w = 1 - d2/r^2: mask = 1 - prod (1 - w).  Pixels are SR_POINTS_TILE square tiles.
+ *   sr_points_silhouette_list_capacity: slots of the tile lists (N * V * tiles per point), SR_EINVAL if invalid.
+ *   sr_points_silhouette_bin: order [N,V] = each frame's point indices in (Z, index) order (a stable sort by Z);
+ *     writes per (frame, rank) a fixed number of slots: tile_keys = n * tiles + tile, tile_points = the point index;
+ *     unused slots hold key N * tiles and point -1.  A stable sort of the keys (carrying tile_points) then gives
+ *     every tile's points in (Z, index) order; tile_offsets [N * tiles + 1] delimit them.
+ *   sr_points_silhouette_forward: mask [N,H,W] plus the backward's per-pixel state: kth_key = (Z bits << 32 | index)
+ *     of the K-th kept point (all ones when fewer than K cover), prod = product of the nonzero (1 - w), zeros = count
+ *     of w == 1.
+ *   sr_points_silhouette_backward: grad_pts [N,V,3] = dL/d(col, row, Z) (Z gets 0) for grad_mask [N,H,W].
+ *     No atomics: bit-identical reruns. */
+#define SR_POINTS_TILE 16
+int64_t sr_points_silhouette_list_capacity(int64_t N, int64_t V, int H, int W, float radius);
+int sr_points_silhouette_bin(const float* pts_screen, const int64_t* order, int64_t N, int64_t V, int H, int W,
+                             float radius, int64_t* tile_keys, int32_t* tile_points, cudaStream_t s);
+int sr_points_silhouette_forward(const float* pts_screen, const int64_t* tile_offsets, const int32_t* tile_points,
+                                 int64_t N, int64_t V, int H, int W, float radius, int K, float* mask,
+                                 uint64_t* kth_key, float* prod, int32_t* zeros, cudaStream_t s);
+int sr_points_silhouette_backward(const float* pts_screen, const float* grad_mask, const uint64_t* kth_key,
+                                  const float* prod, const int32_t* zeros, int64_t N, int64_t V, int H, int W,
+                                  float radius, float* grad_pts, cudaStream_t s);
+
 /* Training half of the tensor-core engine (model/network.py:599-639, 774-796: loss.backward() and the parameter
  * VJPs; in a reverse launch (`mul_tiles` != NULL) `dstash` is an INPUT: the fp32 act'(z) the forward launch of the
  * previous layer wrote (leading dimension = that layer's width rounded up to 256), or NULL to recompute act' from the

@@ -128,6 +128,11 @@ SIGNATURES = {
     "sr_mesh_vertex_normals": (C.c_int, [c_f, c_f, c_f, c_f, i64, i64, i64, c_f, stream_t]),
     "sr_shade_phong": (C.c_int, [c_f, c_f, c_f, c_f, i64, i64, i64, c_f, c_f, i32, i32, c_f, c_f,
                                  C.POINTER(PhongParams), c_f, stream_t]),
+    "sr_points_silhouette_list_capacity": (i64, [i64, i64, i32, i32, f32]),
+    "sr_points_silhouette_bin": (C.c_int, [c_f, c_f, i64, i64, i32, i32, f32, c_f, c_f, stream_t]),
+    "sr_points_silhouette_forward": (C.c_int, [c_f, c_f, c_f, i64, i64, i32, i32, f32, i32, c_f, c_f, c_f, c_f,
+                                               stream_t]),
+    "sr_points_silhouette_backward": (C.c_int, [c_f, c_f, c_f, c_f, c_f, i64, i64, i32, i32, f32, c_f, stream_t]),
     "sr_tc_wgrad_partial_bytes": (i64, [i64, i32, i32, C.POINTER(C.c_int)]),
     "sr_tc_debug_wgrad_desc_swap": (None, [i32]),
     "sr_tc_mlp_forward": (C.c_int, [C.POINTER(TcLayer), i32, c_f, i64, i32, i32, i32, c_f, C.POINTER(C.c_void_p),

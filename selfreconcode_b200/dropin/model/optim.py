@@ -121,7 +121,9 @@ class OptimNetwork(nn.Module):
     # ---- network.py:172-205 -------------------------------------------------------------------
     def update_hierarchical_config(self, device):
         """Applies the hierarchy level queued by utils.set_hierarchical_config at the next remesh: new loss
-        conf, point renderer with the level's radius, hard (blur 0) silhouette rasteriser settings."""
+        conf, point renderer with the level's radius, hard (blur 0) silhouette rasteriser settings.  With the
+        built-in mesh rasteriser (raster.MeshRasterizer) the point renderer is the built-in device one and no
+        pytorch3d is needed; with pytorch3d's rasteriser it is pytorch3d's."""
         if self.next_conf is None:
             return
         self.conf = self.next_conf
@@ -130,7 +132,14 @@ class OptimNetwork(nn.Module):
         self.remesh_intersect = tc.get_int('point_render.remesh_intersect')
         self.sdfShrinkRadius = 0.0
         ras = self.maskRender.rasterizer if self.maskRender is not None else None
-        if ras is not None and hasattr(ras, "raster_settings"):
+        from . import raster
+        if isinstance(ras, raster.MeshRasterizer):
+            H, W = ras.raster_settings.image_size[0], ras.raster_settings.image_size[1]
+            self.pcRender = raster.PointsSilhouetteRenderer(raster.PointsRasterizer(
+                cameras=ras.cameras, raster_settings=raster.PointsRasterizationSettings(
+                    image_size=(H, W), radius=tc.get_float('point_render.radius'), points_per_pixel=50))).to(device)
+            ras.raster_settings = raster.RasterSettings((H, W))
+        elif ras is not None and hasattr(ras, "raster_settings"):
             P = _p3d()
             H, W = ras.raster_settings.image_size[0], ras.raster_settings.image_size[1]
             big = 92 if 1024 < max(H, W) <= 2048 else None
@@ -475,7 +484,7 @@ class OptimNetwork(nn.Module):
 
     def _pc_silhouette_loss(self, defTmpVs, defconds, gtMs, H, W, ratio):
         """network.py:497-507: soft point-cloud silhouette of the deformed template vs the (dilated) gt
-        mask, then computeTmpPcLoss.  Without a point renderer (no pytorch3d, none injected) the term is
+        mask, then computeTmpPcLoss.  Without a point renderer (no level applied yet, none injected) the term is
         unavailable: that is an error unless `allow_missing_pc_loss` is set -- never a silent omission."""
         self.info['pc_loss'] = {}
         if self.pcRender is None:

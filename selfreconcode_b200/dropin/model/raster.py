@@ -7,7 +7,8 @@ binned pytorch3d pipeline, and on the camera convention of RectifiedPerspectiveC
 (pixel centres at integer (col, row)), so no NDC round trip.  `SilhouetteRenderer` is the minimal
 MeshRendererWithFragments: `renderer(verts [N,V,3], faces) -> (hard silhouette [N,H,W,4], fragments)`.
 `MeshRenderer` with `HardPhongShader` is the shaded counterpart OptimNetwork.infer renders with (infer.py:80-90):
-Phong-lit images of the same fragments (csrc/mesh_shade.cu)."""
+Phong-lit images of the same fragments (csrc/mesh_shade.cu).  `PointsSilhouetteRenderer` is the soft point-cloud
+silhouette of the optimisation step (csrc/points_silhouette.cu), with its gradient."""
 import types
 
 import torch
@@ -30,6 +31,19 @@ class RasterSettings:
                                       "blur 0, one face per pixel, no culling, unclipped barycentrics")
 
 
+def screen_vertices(verts, cameras):
+    """[N,V,3] world -> (col, row, view-space depth Z) with frame n seen by camera n (CameraMine.py:138-142);
+    differentiable.  This is RectifiedPerspectiveCameras' NDC projection with pixel (i, j) centred at
+    NDC (1-(2j+1)/W, 1-(2i+1)/H), expressed in pixel units."""
+    N = verts.shape[0]
+    R, T = cameras.R[:N], cameras.T[:N]
+    pc = (verts.unsqueeze(3) * R.unsqueeze(1)).sum(2) + T.view(N, 1, 3)          # p R + T, no GEMM launch
+    f, c = cameras.focal_length[:N], cameras.principal_point[:N]
+    x = c[:, 0:1] - pc[..., 0] * f[:, 0:1] / pc[..., 2]
+    y = c[:, 1:2] - pc[..., 1] * f[:, 1:2] / pc[..., 2]
+    return torch.stack([x, y, pc[..., 2]], dim=-1)
+
+
 class MeshRasterizer:
     def __init__(self, cameras, raster_settings):
         self.cameras = cameras
@@ -41,15 +55,7 @@ class MeshRasterizer:
         return self
 
     def screen_vertices(self, verts, cameras=None):
-        """[N,V,3] world -> (col, row, depth) with frame n seen by camera n (CameraMine.py:138-142)."""
-        cam = cameras if cameras is not None else self.cameras
-        N = verts.shape[0]
-        R, T = cam.R[:N], cam.T[:N]
-        pc = (verts.unsqueeze(3) * R.unsqueeze(1)).sum(2) + T.view(N, 1, 3)          # p R + T, no GEMM launch
-        f, c = cam.focal_length[:N], cam.principal_point[:N]
-        x = c[:, 0:1] - pc[..., 0] * f[:, 0:1] / pc[..., 2]
-        y = c[:, 1:2] - pc[..., 1] * f[:, 1:2] / pc[..., 2]
-        return torch.stack([x, y, pc[..., 2]], dim=-1)
+        return screen_vertices(verts, cameras if cameras is not None else self.cameras)
 
     def __call__(self, verts, faces, cameras=None):
         H, W = self.raster_settings.image_size
@@ -74,6 +80,53 @@ class SilhouetteRenderer:
         frags = self.rasterizer(verts, faces, cameras)
         cover = (frags.pix_to_face >= 0).float()
         return torch.cat([cover.expand(-1, -1, -1, 3), cover], dim=-1), frags
+
+
+# ---- soft point silhouette of the optimisation step (model/network.py:495-505, 647-688) --------------------------
+# pytorch3d's PointsRasterizer + AlphaCompositor(background_color=None) on the deformed template with unit features,
+# restated on the device (csrc/points_silhouette.cu).  Keyword names and defaults are pytorch3d's.
+
+class PointsRasterizationSettings:
+    def __init__(self, image_size, radius=0.01, points_per_pixel=8, bin_size=None):
+        self.image_size = tuple(image_size)
+        self.radius = radius
+        self.points_per_pixel = points_per_pixel
+        self.bin_size = bin_size          # accepted for pytorch3d compatibility; the device kernel bins by itself
+
+
+class PointsRasterizer:
+    def __init__(self, cameras, raster_settings):
+        self.cameras = cameras
+        self.raster_settings = raster_settings
+
+    def to(self, device):
+        if hasattr(self.cameras, "to"):
+            self.cameras = self.cameras.to(device)
+        return self
+
+
+class PointsSilhouetteRenderer:
+    """`masks [N,H,W,1] = renderer(verts [N,V,3])`: the soft silhouette of the N frames' points, each seen by its own
+    camera, differentiable w.r.t. verts.  Takes the tensor directly (no Pointclouds container): OptimNetwork's
+    `takes_tensors` point-renderer protocol."""
+    takes_tensors = True
+
+    def __init__(self, rasterizer):
+        self.rasterizer = rasterizer
+
+    @property
+    def radius(self):
+        return self.rasterizer.raster_settings.radius
+
+    def to(self, device):
+        self.rasterizer.to(device)
+        return self
+
+    def __call__(self, verts, cameras=None):
+        s = self.rasterizer.raster_settings
+        H, W = s.image_size
+        pts = screen_vertices(verts, cameras if cameras is not None else self.rasterizer.cameras)
+        return ops.points_silhouette(pts, H, W, s.radius, s.points_per_pixel)
 
 
 # ---- shaded images of OptimNetwork.infer (model/network.py:318-338; infer.py:90 installs HardPhongShader) ---------

@@ -268,7 +268,9 @@ def DCTSpace(k, N):
 
 def _new_engine(like, resolutions):
     from MCAcc import Seg3dLossless
-    return Seg3dLossless(query_func=None, b_min=like.b_min, b_max=like.b_max, resolutions=resolutions,
+    # the box as host lists (as getOptNet passes it): the engine builds its lattice tensors on the host first
+    return Seg3dLossless(query_func=None, b_min=like.b_min.view(3).tolist(), b_max=like.b_max.view(3).tolist(),
+                         resolutions=resolutions,
                          align_corners=False, balance_value=0.0, visualize=False, debug=False,
                          use_cuda_impl=False, faster=False).to(like.b_min.device)
 

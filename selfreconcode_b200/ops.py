@@ -156,6 +156,77 @@ def shade_phong(verts, normals, faces, pix_to_face, bary, cam_pos, light_pos, pa
 _KERNELS_PER_CALL.update({"mesh_vertex_normals": 1, "shade_phong": 1})
 
 
+POINTS_TILE = 16     # SR_POINTS_TILE: pixels per side of a tile of sr_points_silhouette_forward
+
+
+class _PointsSilhouette(torch.autograd.Function):
+    """Soft point silhouette (csrc/points_silhouette.cu): pytorch3d's PointsRasterizer + AlphaCompositor with unit
+    features, differentiable w.r.t. the (col, row) screen coordinates."""
+
+    @staticmethod
+    def forward(ctx, pts_screen, H, W, radius, K):
+        _need_cuda(pts_screen)
+        vs = pts_screen.detach().contiguous().float()
+        if vs.dim() != 3 or vs.shape[2] != 3:
+            raise ValueError("points_silhouette: pts_screen must be [N,V,3]")
+        N, V, _ = vs.shape
+        lib = _lib.load()
+        cap = lib.sr_points_silhouette_list_capacity(N, V, H, W, radius)
+        if cap < 0:
+            raise ValueError("points_silhouette: invalid sizes / radius (N=%d V=%d H=%d W=%d r=%r K=%d)"
+                             % (N, V, H, W, radius, K))
+        if K <= 0:
+            raise ValueError("points_silhouette: points_per_pixel must be positive")
+        dev = vs.device
+        tiles = ((H + POINTS_TILE - 1) // POINTS_TILE) * ((W + POINTS_TILE - 1) // POINTS_TILE)
+        with torch.cuda.device(dev):
+            z = vs[..., 2]
+            # each frame's points in (Z, index) order: a stable sort keeps equal depths in index order
+            order = torch.sort(torch.where(z >= 0, z, torch.full_like(z, math.inf)), dim=1, stable=True).indices
+            keys = torch.empty(cap, dtype=torch.int64, device=dev)
+            ids = torch.empty(cap, dtype=torch.int32, device=dev)
+            check(lib.sr_points_silhouette_bin(_p(vs), _p(order), N, V, H, W, radius, _p(keys), _p(ids), _stream()),
+                  "points_silhouette_bin")
+            keys, perm = torch.sort(keys, stable=True)       # tile-major, (Z, index) order kept inside each tile
+            ids = ids[perm]
+            offsets = torch.searchsorted(keys, torch.arange(N * tiles + 1, dtype=torch.int64, device=dev))
+            mask = torch.empty((N, H, W, 1), dtype=torch.float32, device=dev)
+            kth = torch.empty((N, H, W), dtype=torch.int64, device=dev)
+            prod = torch.empty((N, H, W), dtype=torch.float32, device=dev)
+            zeros = torch.empty((N, H, W), dtype=torch.int32, device=dev)
+            check(lib.sr_points_silhouette_forward(_p(vs), _p(offsets), _p(ids), N, V, H, W, radius, K, _p(mask),
+                                                   _p(kth), _p(prod), _p(zeros), _stream()),
+                  "points_silhouette_forward")
+        ctx.save_for_backward(vs, kth, prod, zeros)
+        ctx.args = (H, W, radius)
+        ctx.in_dtype = pts_screen.dtype
+        return mask
+
+    @staticmethod
+    def backward(ctx, grad_mask):
+        vs, kth, prod, zeros = ctx.saved_tensors
+        H, W, radius = ctx.args
+        N, V, _ = vs.shape
+        g = grad_mask.contiguous().float()
+        out = torch.empty_like(vs)
+        with torch.cuda.device(vs.device):
+            check(_lib.load().sr_points_silhouette_backward(_p(vs), _p(g), _p(kth), _p(prod), _p(zeros), N, V, H, W,
+                                                            radius, _p(out), _stream()),
+                  "points_silhouette_backward")
+        return out.to(ctx.in_dtype), None, None, None, None
+
+
+def points_silhouette(pts_screen, H, W, radius, K):
+    """pts_screen [N,V,3] = (col, row, view-space Z) per frame (raster.screen_vertices), radius in NDC units,
+    K points per pixel -> soft silhouette [N,H,W,1] (pytorch3d 0.4.0 PointsRasterizer + AlphaCompositor, unit
+    features); differentiable w.r.t. (col, row).  DESIGN.md section 3.3."""
+    return _PointsSilhouette.apply(pts_screen, int(H), int(W), float(radius), int(K))
+
+
+_KERNELS_PER_CALL.update({"points_silhouette_bin": 1, "points_silhouette_forward": 1,
+                          "points_silhouette_backward": 1})
+
+
 def svals3x3(J, want_v=True):
     """J [n,3,3] f32 CUDA -> (singular values [n,3] descending, V [n,3,3] | None)."""
     _need_cuda(J)
