@@ -360,6 +360,31 @@ int sr_points_silhouette_backward(const float* pts_screen, const float* grad_mas
                                   const float* prod, const int32_t* zeros, int64_t N, int64_t V, int H, int W,
                                   float radius, float* grad_pts, cudaStream_t s);
 
+/* Texture atlas of the reconstruction (texture_mesh_extract.py:57-144: VideoAvatar's Isomapper aggregation), over the
+ * T atlas texels a UV face covers (the UV raster: sr_raster_mesh on the atlas), S <= SR_TEXTURE_MAX_SLOTS slots each.
+ * Slots are slot-major: slot_rgb [S][3][T] (colour in [0,1], planar), slot_alpha [S][T] (c0 = cos(max_angle) when
+ * empty), slot_view [S][T] (frame id, -1 when empty); min_alpha / min_slot [T] = the smallest slot alpha and the first
+ * slot holding it (start: c0, 0).
+ *   sr_texture_accumulate: one frame.  texel_face [T] (face of F), texel_bary [T,3]; verts_screen [V,3] = the frame's
+ *     (col, row, Z), pixel centres at integers; vert_weight [V] = max(0, -n_v . d_v); face_usable [F] (0/1); image
+ *     [H,W,3] uint8 in its own channel order.  alpha = sum b_i w_i over a usable face (0 otherwise); when alpha >
+ *     min_alpha the slot min_slot takes (bilinear(image, sum b_i s_i) / 255 with clamp-to-edge, alpha, frame_id >= 0)
+ *     and the pair is rescanned.
+ *   sr_texture_finish: count = #slots with alpha > c0, mask_final = count >= min_views, view_id = frame of the first slot
+ *     with the largest alpha (-1 unless mask_final), tex_median = per-channel median of the filled slots (mean of the two
+ *     middle values for an even count; 0 unless mask_final).  Written at texel_index [T] of the outputs tex_median
+ *     [R*R,3], mask_final / view_id / count [R*R]; other texels are left as they are.
+ * One thread owns each texel (no atomics: bit-identical reruns). */
+#define SR_TEXTURE_MAX_SLOTS 64
+int sr_texture_accumulate(int64_t T, int S, const int32_t* texel_face, const float* texel_bary,
+                          const float* verts_screen, const int64_t* faces, int64_t V, int64_t F, const float* vert_weight,
+                          const uint8_t* face_usable, const uint8_t* image, int H, int W, int frame_id,
+                          float* slot_rgb, float* slot_alpha, int32_t* slot_view, float* min_alpha, int32_t* min_slot,
+                          cudaStream_t s);
+int sr_texture_finish(int64_t T, int S, const int64_t* texel_index, const float* slot_rgb, const float* slot_alpha,
+                      const int32_t* slot_view, float c0, int min_views, float* tex_median, uint8_t* mask_final,
+                      int32_t* view_id, int32_t* count, cudaStream_t s);
+
 /* Training half of the tensor-core engine (model/network.py:599-639, 774-796: loss.backward() and the parameter
  * VJPs; in a reverse launch (`mul_tiles` != NULL) `dstash` is an INPUT: the fp32 act'(z) the forward launch of the
  * previous layer wrote (leading dimension = that layer's width rounded up to 256), or NULL to recompute act' from the

@@ -133,6 +133,9 @@ SIGNATURES = {
     "sr_points_silhouette_forward": (C.c_int, [c_f, c_f, c_f, i64, i64, i32, i32, f32, i32, c_f, c_f, c_f, c_f,
                                                stream_t]),
     "sr_points_silhouette_backward": (C.c_int, [c_f, c_f, c_f, c_f, c_f, i64, i64, i32, i32, f32, c_f, stream_t]),
+    "sr_texture_accumulate": (C.c_int, [i64, i32, c_f, c_f, c_f, c_f, i64, i64, c_f, c_f, c_f, i32, i32, i32, c_f, c_f,
+                                        c_f, c_f, c_f, stream_t]),
+    "sr_texture_finish": (C.c_int, [i64, i32, c_f, c_f, c_f, c_f, f32, i32, c_f, c_f, c_f, c_f, stream_t]),
     "sr_tc_wgrad_partial_bytes": (i64, [i64, i32, i32, C.POINTER(C.c_int)]),
     "sr_tc_debug_wgrad_desc_swap": (None, [i32]),
     "sr_tc_mlp_forward": (C.c_int, [C.POINTER(TcLayer), i32, c_f, i64, i32, i32, i32, c_f, C.POINTER(C.c_void_p),

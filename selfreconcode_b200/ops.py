@@ -227,6 +227,47 @@ _KERNELS_PER_CALL.update({"points_silhouette_bin": 1, "points_silhouette_forward
                           "points_silhouette_backward": 1})
 
 
+TEXTURE_MAX_SLOTS = 64     # SR_TEXTURE_MAX_SLOTS
+
+
+def texture_accumulate(texel_face, texel_bary, verts_screen, faces, vert_weight, face_usable, image, frame_id, slots):
+    """One frame into the texture slots (csrc/texture_bake.cu).  texel_face [T] int32, texel_bary [T,3] of the covered
+    atlas texels; verts_screen [V,3] (col, row, Z); faces [F,3] int64; vert_weight [V]; face_usable [F] uint8; image
+    [H,W,3] uint8; slots = dict(rgb [S,3,T], alpha [S,T], view [S,T] int32, min_alpha [T], min_slot [T] int32),
+    updated in place."""
+    _need_cuda(texel_face, texel_bary, verts_screen, faces, vert_weight, face_usable, image)
+    S, T = slots["alpha"].shape
+    V, F = verts_screen.shape[0], faces.shape[0]
+    H, W = image.shape[0], image.shape[1]
+    if image.dim() != 3 or image.shape[2] != 3 or image.dtype != torch.uint8:
+        raise ValueError("texture_accumulate: image must be [H,W,3] uint8")
+    if texel_face.numel() != T or texel_bary.numel() != 3 * T or vert_weight.numel() != V or face_usable.numel() != F:
+        raise ValueError("texture_accumulate: inconsistent shapes")
+    with torch.cuda.device(image.device):
+        check(_lib.load().sr_texture_accumulate(
+            T, S, _p(texel_face), _p(texel_bary), _p(verts_screen), _p(faces), V, F, _p(vert_weight), _p(face_usable),
+            _p(image), int(H), int(W), int(frame_id), _p(slots["rgb"]), _p(slots["alpha"]), _p(slots["view"]),
+            _p(slots["min_alpha"]), _p(slots["min_slot"]), _stream()), "texture_accumulate")
+
+
+def texture_finish(texel_index, slots, c0, min_views, n_texels):
+    """count / mask_final / view_id / per-channel median of the filled slots at the covered texels texel_index [T]
+    int64 of an atlas of n_texels -> (tex_median [n,3] float32, mask_final [n] uint8, view_id [n] int32, count [n]
+    int32); texels outside texel_index get 0 / 0 / -1 / 0."""
+    _need_cuda(texel_index)
+    S, T = slots["alpha"].shape
+    dev = texel_index.device
+    med = torch.zeros((n_texels, 3), dtype=torch.float32, device=dev)
+    mask = torch.zeros(n_texels, dtype=torch.uint8, device=dev)
+    view = torch.full((n_texels,), -1, dtype=torch.int32, device=dev)
+    count = torch.zeros(n_texels, dtype=torch.int32, device=dev)
+    with torch.cuda.device(dev):
+        check(_lib.load().sr_texture_finish(T, S, _p(texel_index), _p(slots["rgb"]), _p(slots["alpha"]),
+                                            _p(slots["view"]), float(c0), int(min_views), _p(med), _p(mask), _p(view),
+                                            _p(count), _stream()), "texture_finish")
+    return med, mask, view, count
+
+
 def svals3x3(J, want_v=True):
     """J [n,3,3] f32 CUDA -> (singular values [n,3] descending, V [n,3,3] | None)."""
     _need_cuda(J)
