@@ -57,7 +57,9 @@ struct Step {
   uint32_t bytes;
   int nslices;
 };
-constexpr int kMaxSteps = 40;
+// The longest program is trace_rev_kernel's: forward and backward sweeps of the SDF and the translator, each up to
+// SR_MLP_MAX_LAYERS steps.  program_add_* does not check the bound, so this must cover it.
+constexpr int kMaxSteps = 4 * SR_MLP_MAX_LAYERS;
 
 struct Smem {
   float* at;        // [kMaxK][kRowStride]
@@ -467,9 +469,12 @@ __device__ __forceinline__ void bwd_epilogue(const Smem& s, const sr_mlp_desc& n
         *reinterpret_cast<float4*>(dst + 4) = make_float4(o[4] * d1.x, o[5] * d1.y, o[6] * d1.z, o[7] * d1.w);
       } else {
         if (skip && col < n_prev + net.d_in && col - n_prev < kStashMax) {
+          // accumulate: every skip layer adds its share of the embedded input's gradient
           float* sg = s.stash + (size_t)(col - n_prev) * kRowStride + 8 * rg;
-          *reinterpret_cast<float4*>(sg) = make_float4(o[0], o[1], o[2], o[3]);
-          *reinterpret_cast<float4*>(sg + 4) = make_float4(o[4], o[5], o[6], o[7]);
+          const float4 s0 = *reinterpret_cast<const float4*>(sg);
+          const float4 s1 = *reinterpret_cast<const float4*>(sg + 4);
+          *reinterpret_cast<float4*>(sg) = make_float4(s0.x + o[0], s0.y + o[1], s0.z + o[2], s0.w + o[3]);
+          *reinterpret_cast<float4*>(sg + 4) = make_float4(s1.x + o[4], s1.y + o[5], s1.z + o[6], s1.w + o[7]);
         }
         if (col < next_k) {  // k-padding of the next backward GEMM
           float* dst = s.at + (size_t)col * kRowStride + 8 * rg;

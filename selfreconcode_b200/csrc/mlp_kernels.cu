@@ -29,6 +29,7 @@ enum {
 };
 constexpr size_t kAuxBytes = (size_t)kTileRows * kAuxStride * 4;
 constexpr size_t kDynSmem = kSmemBytes + kAuxBytes + 256 /*row_pt*/ + 128 /*align*/;
+static_assert(kDynSmem <= 232448, "exceeds the H100's 227 KB of dynamic shared memory per block");
 
 struct TileCtx {
   Smem s;
@@ -961,6 +962,7 @@ __global__ void __launch_bounds__(256) small_layer_kernel(const __grid_constant_
     float v = z[t];
     if (a.act == SR_ACT_SOFTPLUS100) { float d; v = softplus100(v, d); }
     else if (a.act == SR_ACT_RELU) v = fmaxf(v, 0.f);
+    else if (a.act == SR_ACT_TANH) v = tanhf(v);
     if (a.out) a.out[(size_t)(p0 + p) * a.ld_out + col] = v;
     if (a.sdf && col == 0) a.sdf[a.index[p0 + p]] = v;
   }

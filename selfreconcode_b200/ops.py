@@ -1109,6 +1109,10 @@ def _tc_backward_sweep(lib, tcn, cot, bufs, acts, P, m_dev, g_out, g_skip, n_kee
     """cotangent rows `cot` [P][32] of the net outputs -> d/d(embedded input) in g_out [P][ld]
     (first n_keep columns), skip-connection part in g_skip.  acts = the forward sweep's tiles; bufs = a pair of
     staging tile buffers the layers alternate between."""
+    if sum(ly["skip"] for ly in tcn.layers) > 1:
+        # each skip layer's launch stores its input-gradient part into g_skip, so a second one would overwrite the first
+        raise RuntimeError("selfrecon_b200: the tensor-core reverse sweep takes at most one skip layer; "
+                           "use the fp32 engine (trace mode 'reverse', shade_geometry) for this network")
     d_in = tcn.fused.desc.d_in
     cur, nxt = bufs
     check(lib.sr_tc_pack_rows(_p(cot), P, 32, 32, _p(cur), _p(m_dev), _stream()), "tc_pack_rows")

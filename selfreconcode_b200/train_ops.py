@@ -35,6 +35,9 @@ class MlpConfig:
     def __init__(self, acts, skips, d_in, ch, packs=None):
         self.acts = [int(a) for a in acts]
         self.skips = [bool(s) for s in skips]
+        if sum(self.skips) > 1:
+            # sr_tc_mlp_backward stores each skip layer's input-gradient part into one buffer: a second would overwrite it
+            raise RuntimeError("TcMlpFunction: at most one skip layer (got %d)" % sum(self.skips))
         self.d_in = int(d_in)          # width of the embedded input that a skip layer re-appends
         self.ch = int(ch)
         # optional: the module's persistent tensor-core packs (ops.TcNet.layers: W, Wb = W^T, padded bias) of the
