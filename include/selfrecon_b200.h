@@ -385,6 +385,26 @@ int sr_texture_finish(int64_t T, int S, const int64_t* texel_index, const float*
                       const int32_t* slot_view, float c0, int min_views, float* tex_median, uint8_t* mask_final,
                       int32_t* view_id, int32_t* count, cudaStream_t s);
 
+/* Skin-weight volume of a new sequence (model/Deformer.py:235-284, utils/LBSWsmpl.py:2-52: compute_lbswField and
+ * smooth_weights).  Volumes are [C][D][H][W] float (x fastest), (W, H, D) = the resolutions; bmin / bmax are HOST [3].
+ *   sr_lbsw_knn_blend: verts [V,3], vert_ws [V,C].  Voxel (i, j, l) has the centre u * (hi - lo) + lo with
+ *     u = i / W + (1 / W) / 2 (i / (W - 1) with align_corners), every fp32 operation rounded on its own (no FMA).  Its
+ *     k nearest vertices by exact fp32 differences, ordered by (d^2, index), are blended with w_n = 1 / min(max(d_n,
+ *     1e-4), 1) normalised by their sum: field[c] = sum_n w_n vert_ws[idx_n, c] in ascending distance order.
+ *     centres [W*H*D,3] (may be NULL) receives the voxel centres.  1 <= k <= min(V, SR_LBSW_MAX_K),
+ *     1 <= C <= SR_LBSW_MAX_C.
+ *   sr_lbsw_smooth_pass: one Jacobi pass src -> dst (distinct buffers): interior voxels become (c - mean) * 0.7 + mean,
+ *     mean = the six neighbours of src in the order (+z, -z, +y, -y, +x, -x) / 6; boundary voxels keep theirs; every
+ *     voxel is divided by its channel sum; with cut > 0, values below cut become 0.
+ *   sr_lbsw_cut: field[t] < cut -> 0 in place over n values (the utils.LBSWsmpl variant with no smoothing pass).
+ * No atomics: bit-identical reruns. */
+#define SR_LBSW_MAX_K 32
+#define SR_LBSW_MAX_C 32
+int sr_lbsw_knn_blend(const float* verts, const float* vert_ws, int V, int C, const float* bmin, const float* bmax,
+                      int W, int H, int D, int align_corners, int k, float* field, float* centres, cudaStream_t s);
+int sr_lbsw_smooth_pass(const float* src, float* dst, int C, int D, int H, int W, float cut, cudaStream_t s);
+int sr_lbsw_cut(float* field, int64_t n, float cut, cudaStream_t s);
+
 /* Training half of the tensor-core engine (model/network.py:599-639, 774-796: loss.backward() and the parameter
  * VJPs; in a reverse launch (`mul_tiles` != NULL) `dstash` is an INPUT: the fp32 act'(z) the forward launch of the
  * previous layer wrote (leading dimension = that layer's width rounded up to 256), or NULL to recompute act' from the

@@ -350,6 +350,9 @@ def smooth_weights(weights, times=3):
     return weights
 
 
+smooth_weights.lbsw_cut = 0.0
+
+
 def compute_lbswField(bmins, bmaxs, resolutions, smpl_verts, smpl_ws, align_corners=False,
                       mean_neighbor=5, smooth_times=30):
     """model/Deformer.py:246-284 (the copy getOptNet's initialiser uses: no small-weight cut)."""

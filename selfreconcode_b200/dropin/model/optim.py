@@ -173,20 +173,7 @@ class OptimNetwork(nn.Module):
             batches = list(zip(torch.split(vs[perm], 5000), torch.split(ns[perm], 5000)))
             for bi, (on_pts, normals) in enumerate(batches):
                 off_pts = utils.sample_points(on_pts, 1.8, 0.01)
-                on_pts = on_pts.detach().requires_grad_()
-                off_pts.requires_grad_()
-                on_pred = net(on_pts, -1)
-                off_pred = net(off_pts, -1)
-                on_grad = net.gradient(on_pts, on_pred)
-                off_grad = net.gradient(off_pts, off_pred)
-                mnfld_loss = on_pred.abs().mean()
-                grad_loss = ((off_grad.norm(2, dim=-1) - 1) ** 2).mean()
-                loss = mnfld_loss + 0.1 * grad_loss
-                if with_normals:
-                    normals_loss = (on_grad - normals.view(-1, 3).to(on_grad.dtype)).abs().norm(2, dim=1).mean()
-                    loss = loss + 1.0 * normals_loss
-                else:
-                    normals_loss = torch.zeros(1)
+                loss, mnfld_loss, grad_loss, normals_loss = self.igr_losses(on_pts, off_pts, normals, with_normals)
                 opt.zero_grad()
                 loss.backward()
                 opt.step()
@@ -197,6 +184,34 @@ class OptimNetwork(nn.Module):
             sched.step()
         if save_name:
             torch.save(net.state_dict(), save_name)
+
+    def igr_losses(self, on_pts, off_pts, normals, with_normals):
+        """One IGR batch -> (loss, manifold, eikonal, normal term) (network.py:243-270).  With the stock SDF module the
+        on- and off-surface points go through ONE tensor-core forward_train call with grad f as a forward-mode output,
+        so loss.backward() is one reverse sweep plus the weight-gradient GEMMs; otherwise the reference's autograd
+        loop (create_graph=True, then a double backward)."""
+        net = self.sdf
+        n_on = on_pts.shape[0]
+        if hasattr(net, "_train_ok") and net._train_ok():
+            f, g, _ = net.forward_train(torch.cat([on_pts.detach(), off_pts.detach()]), -1, want_grad=True,
+                                        want_feat=False)
+            on_pred, on_grad, off_grad = f[:n_on], g[:n_on], g[n_on:]
+        else:
+            on_pts = on_pts.detach().requires_grad_()
+            off_pts = off_pts.detach().requires_grad_()
+            on_pred = net(on_pts, -1)
+            off_pred = net(off_pts, -1)
+            on_grad = net.gradient(on_pts, on_pred)
+            off_grad = net.gradient(off_pts, off_pred)
+        mnfld_loss = on_pred.abs().mean()
+        grad_loss = ((off_grad.norm(2, dim=-1) - 1) ** 2).mean()
+        loss = mnfld_loss + 0.1 * grad_loss
+        if with_normals:
+            normals_loss = (on_grad - normals.view(-1, 3).to(on_grad.dtype)).abs().norm(2, dim=1).mean()
+            loss = loss + 1.0 * normals_loss
+        else:
+            normals_loss = torch.zeros(1)
+        return loss, mnfld_loss, grad_loss, normals_loss
 
     # ---- network.py:292-302 -------------------------------------------------------------------
     def discretizeSDF(self, ratio, engine=None, balance_value=0.):

@@ -1,8 +1,9 @@
 """Skin-weight volume from a posed SMPL mesh (reference: utils/LBSWsmpl.py:1-52; one-time
 initialiser, SURVEY.md section 8f-4).  For every voxel centre of the box: inverse-distance blend of the
 skin weights of its `mean_neighbor` nearest SMPL vertices, then `smooth_times` damped 6-neighbour
-smoothing passes with per-voxel renormalisation.  Distances go through one fused cdist + top-k per
-chunk on the device the vertices live on."""
+smoothing passes with per-voxel renormalisation.  On CUDA float32 inputs with k and C up to 32 the blend runs on the
+device kernels of csrc/lbsw_field.cu (exact difference norms, ties to the lower index), and so does the smoothing
+when `smooth` is one of the two stock smoothers; other inputs take one cdist + top-k per chunk."""
 import torch
 
 
@@ -17,6 +18,9 @@ def smooth_weights(weights, times=3):
         weights = weights / weights.sum(1, keepdim=True)
     weights[weights < 5.e-3] = 0.0
     return weights
+
+
+smooth_weights.lbsw_cut = 5.e-3     # the device smoother's final cut (0: model.Deformer's variant, no cut)
 
 
 def voxel_centres(bmins, bmaxs, resolutions, device, align_corners=False):
@@ -34,6 +38,14 @@ def voxel_centres(bmins, bmaxs, resolutions, device, align_corners=False):
 
 def compute_lbswField(bmins, bmaxs, resolutions, smpl_verts, smpl_ws, align_corners=False, mean_neighbor=5,
                       smooth_times=30, chunk=50000, smooth=smooth_weights):
+    if (smpl_verts.is_cuda and smpl_verts.dtype == torch.float32 and smpl_ws.dtype == torch.float32
+            and mean_neighbor <= 32 and smpl_ws.shape[-1] <= 32):
+        from selfreconcode_b200 import ops
+        field = ops.lbsw_field(bmins, bmaxs, resolutions, smpl_verts, smpl_ws, align_corners, mean_neighbor)
+        cut = getattr(smooth, "lbsw_cut", None)
+        if cut is None:
+            return smooth(field, smooth_times)
+        return ops.lbsw_smooth(field, smooth_times, cut)
     W, H, D = [int(r) for r in resolutions]
     pts = voxel_centres(bmins, bmaxs, resolutions, smpl_verts.device, align_corners)
     out = []

@@ -268,6 +268,56 @@ def texture_finish(texel_index, slots, c0, min_views, n_texels):
     return med, mask, view, count
 
 
+LBSW_MAX_K = 32           # SR_LBSW_MAX_K
+LBSW_MAX_C = 32           # SR_LBSW_MAX_C
+
+
+def lbsw_field(bmins, bmaxs, resolutions, verts, vert_ws, align_corners=False, k=5, want_centres=False):
+    """Inverse-distance blend of the skin weights of the k nearest vertices at every voxel centre (csrc/lbsw_field.cu):
+    verts [V,3], vert_ws [V,C] float32 CUDA, (W,H,D) = resolutions -> field [1,C,D,H,W] (and the voxel centres
+    [W*H*D,3], x fastest, with want_centres).  The centres are bit-identical to utils.LBSWsmpl.voxel_centres."""
+    _need_cuda(verts, vert_ws)
+    if verts.dtype != torch.float32 or vert_ws.dtype != torch.float32:
+        raise ValueError("lbsw_field: verts and vert_ws must be float32")
+    verts = verts.reshape(-1, 3).contiguous()
+    V, Cc = verts.shape[0], vert_ws.shape[-1]
+    vert_ws = vert_ws.reshape(V, Cc).contiguous()
+    W, H, D = [int(r) for r in resolutions]
+    lo = (C.c_float * 3)(*torch.as_tensor(bmins, dtype=torch.float32).reshape(3).tolist())
+    hi = (C.c_float * 3)(*torch.as_tensor(bmaxs, dtype=torch.float32).reshape(3).tolist())
+    field = torch.empty((1, Cc, D, H, W), dtype=torch.float32, device=verts.device)
+    centres = torch.empty((W * H * D, 3), dtype=torch.float32, device=verts.device) if want_centres else None
+    with torch.cuda.device(verts.device):
+        check(_lib.load().sr_lbsw_knn_blend(_p(verts), _p(vert_ws), V, Cc, lo, hi, W, H, D, int(bool(align_corners)),
+                                            int(k), _p(field), _p(centres), _stream()), "lbsw_knn_blend")
+    return (field, centres) if want_centres else field
+
+
+def lbsw_smooth(field, times, cut=0.0):
+    """`times` Jacobi passes of the damped 6-neighbour smoother with per-voxel renormalisation over field [1,C,D,H,W]
+    float32 CUDA (two buffers in ping-pong, one launch per pass); with cut > 0, values below it become 0 after the last
+    pass (after the blend itself when times == 0).  Returns a new volume; `field` is not modified."""
+    _need_cuda(field)
+    if field.dtype != torch.float32 or field.dim() != 5 or field.shape[0] != 1:
+        raise ValueError("lbsw_smooth: field must be [1,C,D,H,W] float32")
+    _, Cc, D, H, W = field.shape
+    lib = _lib.load()
+    src = field.contiguous()
+    with torch.cuda.device(field.device):
+        if times <= 0:
+            src = src.clone()
+            if cut > 0:
+                check(lib.sr_lbsw_cut(_p(src), src.numel(), float(cut), _stream()), "lbsw_cut")
+            return src
+        bufs = [torch.empty_like(src), torch.empty_like(src) if times > 1 else None]
+        for t in range(times):
+            dst = bufs[t % 2]
+            check(lib.sr_lbsw_smooth_pass(_p(src), _p(dst), Cc, D, H, W, float(cut) if t == times - 1 else 0.0,
+                                          _stream()), "lbsw_smooth_pass")
+            src = dst
+    return src
+
+
 def svals3x3(J, want_v=True):
     """J [n,3,3] f32 CUDA -> (singular values [n,3] descending, V [n,3,3] | None)."""
     _need_cuda(J)
