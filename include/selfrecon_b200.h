@@ -429,10 +429,18 @@ int sr_tc_unpack_rows(const void* T, int64_t M, int K, int Kpad, float* out, int
  * columns = the embedded input) -> out [M, n_out] (n_out = 0: all n_last columns); a skip layer's input is
  * cat(previous output, x0[:, :d_in]) / sqrt(2).  Keeps the input tiles (A_in), every hidden layer's activation tiles
  * (acts[i], sr_tc_act_bytes(M, k_{i+1})) and, for softplus layers, the fp32 act'(z) (stashes[i] [M, pad256(n_i)] or
- * NULL).  m_dev (may be NULL): device-side row count <= M (active rays).  backward: gout [M, n_last] -> dW[l] [n,k] / db[l] [n] (NULL entries are
- * skipped) and x0_grad [M, ld] (or NULL); D0 / D1 = two delta tile buffers of sr_tc_act_bytes(M, widest layer),
- * part = sr_tc_wgrad_partial_bytes scratch, the largest over the layers' (Kd, Kx) pairs, colsum_ws = colsum_slices x widest floats,
- * g_skip [M, g_skip_ld] scratch when a layer has a skip connection. */
+ * NULL).  m_dev (may be NULL): device-side row count <= M (active rays).  backward: the one reverse sweep, from
+ * gout [M, gout_ld] (gout_ld >= n_last; its first n_last columns are the cotangent) -> dW[l] [n,k] / db[l] [n] (dW / db
+ * may be NULL arrays, NULL entries are skipped) and x0_grad [M, ld] (or NULL); D0 / D1 = two delta tile buffers of
+ * sr_tc_act_bytes(M, widest layer); only when some dW[l] / db[l] is requested: A_in = the forward's input tiles,
+ * part = sr_tc_wgrad_partial_bytes scratch, the largest over the layers' (Kd, Kx) pairs, colsum_ws = colsum_slices x
+ * widest floats.  g_skip [M, g_skip_ld] receives the skip layer's part of the input gradient (its first d_in columns)
+ * when a layer has a skip connection; more than one skip layer returns SR_EUNSUPPORTED.  The input layer's launch writes
+ * the first n_keep columns of x0_grad: Wb_head = NULL takes layers[0].Wb with n_keep = layers[0].k, otherwise Wb_head =
+ * sr_tc_pack_weights of the first n_keep rows of W^T (a narrow launch when n_keep <= 64).  fold_skip = 1 then zeroes
+ * columns [n_keep, ld) of x0_grad and adds g_skip into its first d_in columns; fold_skip = 0 leaves the skip part in
+ * g_skip (sr_tc_embed_backward and sr_tc_trace_update take it as an input) and launches nothing after that layer.
+ * m_dev (may be NULL) is passed to the pack and every layer launch; it requires no dW / db and fold_skip = 0. */
 typedef struct sr_tc_layer {
   const void* W;          /* packed weights, forward orientation (sr_tc_pack_weights of [n,k]) */
   const void* Wb;         /* packed W^T ([k,n]) for the reverse launch */
@@ -444,9 +452,10 @@ int sr_tc_mlp_forward(const sr_tc_layer* layers, int L, const float* x0, int64_t
                       void* const* acts, float* const* stashes, float* out, const int32_t* m_dev, int n_out,
                       cudaStream_t s);
 int sr_tc_mlp_backward(const sr_tc_layer* layers, int L, int64_t M, int ld, int d_in, int ch, const float* gout,
-                       const void* A_in, void* const* acts, float* const* stashes, void* D0, void* D1, float* part,
-                       float* colsum_ws, int colsum_slices, float* const* dW, float* const* db, float* x0_grad,
-                       float* g_skip, int g_skip_ld, cudaStream_t s);
+                       int gout_ld, const void* A_in, void* const* acts, float* const* stashes, void* D0, void* D1,
+                       float* part, float* colsum_ws, int colsum_slices, float* const* dW, float* const* db,
+                       float* x0_grad, float* g_skip, int g_skip_ld, const void* Wb_head, int n_keep, int fold_skip,
+                       const int32_t* m_dev, cudaStream_t s);
 
 /* Batched 3x3 singular values (descending) + right singular vectors (columns of V, may be NULL), and the
  * backward of a function of the VALUES: gJ = sum_i gS_i u_i v_i^T.  Replaces `torch.svd(Jacobs.cpu())` of the
@@ -490,8 +499,8 @@ int sr_sdf_forward_small(const sr_mlp_desc* net, const float* pts, int64_t P, co
                          const int32_t* m_dev, float* sdf, void* work, int cap, cudaStream_t s);
 
 /* Pointwise stages of the tensor-core tracer (one OptimizeSurfacePs iteration =
- * embed -> sr_tc_mlp_forward (activations kept per layer) -> sr_tc_trace_mid -> sr_tc_linear x
- * layers (reverse sweep, mul_tiles = the forward activations) -> sr_tc_trace_update).  All take an optional active
+ * embed -> sr_tc_mlp_forward (activations kept per layer) -> sr_tc_trace_mid -> sr_tc_mlp_backward
+ * (reverse sweep over the forward activations, fold_skip = 0) -> sr_tc_trace_update).  All take an optional active
  * list + device-side count so the host never synchronises.  pw_s / pw_d are HOST arrays. */
 int sr_tc_trace_mid(const int32_t* index, const int32_t* m_dev, int64_t P, const float* pts,
                     const float* rays, const int64_t* batch_inds, const float* f, const float* off,

@@ -144,9 +144,10 @@ SIGNATURES = {
     "sr_tc_debug_wgrad_desc_swap": (None, [i32]),
     "sr_tc_mlp_forward": (C.c_int, [C.POINTER(TcLayer), i32, c_f, i64, i32, i32, i32, c_f, C.POINTER(C.c_void_p),
                                     C.POINTER(C.c_void_p), c_f, c_f, i32, stream_t]),
-    "sr_tc_mlp_backward": (C.c_int, [C.POINTER(TcLayer), i32, i64, i32, i32, i32, c_f, c_f, C.POINTER(C.c_void_p),
-                                     C.POINTER(C.c_void_p), c_f, c_f, c_f, c_f, i32, C.POINTER(C.c_void_p),
-                                     C.POINTER(C.c_void_p), c_f, c_f, i32, stream_t]),
+    "sr_tc_mlp_backward": (C.c_int, [C.POINTER(TcLayer), i32, i64, i32, i32, i32, c_f, i32, c_f,
+                                     C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), c_f, c_f, c_f, c_f, i32,
+                                     C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), c_f, c_f, i32, c_f, i32, i32, c_f,
+                                     stream_t]),
     "sr_tc_wgrad": (C.c_int, [c_f, i32, c_f, i32, i64, c_f, c_f, i32, i32, i32, stream_t]),
     "sr_tc_colsum": (C.c_int, [c_f, i64, i32, i32, c_f, i32, stream_t]),
     "sr_tc_unpack_rows": (C.c_int, [c_f, i64, i32, i32, c_f, i32, stream_t]),

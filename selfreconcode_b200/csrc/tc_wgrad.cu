@@ -381,28 +381,40 @@ int sr_tc_mlp_forward(const sr_tc_layer* layers, int L, const float* x0, int64_t
 }
 
 int sr_tc_mlp_backward(const sr_tc_layer* layers, int L, int64_t M, int ld, int d_in, int ch, const float* gout,
-                       const void* A_in, void* const* acts, float* const* stashes, void* D0, void* D1, float* part,
-                       float* colsum_ws, int colsum_slices, float* const* dW, float* const* db, float* x0_grad,
-                       float* g_skip, int g_skip_ld, cudaStream_t s) {
+                       int gout_ld, const void* A_in, void* const* acts, float* const* stashes, void* D0, void* D1,
+                       float* part, float* colsum_ws, int colsum_slices, float* const* dW, float* const* db,
+                       float* x0_grad, float* g_skip, int g_skip_ld, const void* Wb_head, int n_keep, int fold_skip,
+                       const int32_t* m_dev, cudaStream_t s) {
   using namespace sr_tc;
-  if (!layers || L <= 0 || L > 16 || M <= 0 || !gout || !A_in || !D0 || !D1 || !part || !colsum_ws || !dW || !db)
-    return SR_EINVAL;
+  if (!layers || L <= 0 || L > 16 || M <= 0 || !gout || !D0 || !D1 || (L > 1 && !acts)) return SR_EINVAL;
   const int n_last = layers[L - 1].n;
+  int n_skip = 0;
+  bool params = false;
+  for (int l = 0; l < L; ++l) {
+    n_skip += layers[l].skip != 0;
+    params |= (dW && dW[l]) || (db && db[l]);
+  }
+  // each skip layer's reverse launch stores (does not add) its part of the input gradient into g_skip
+  if (n_skip > 1) return SR_EUNSUPPORTED;
+  // rows past m_dev hold stale tiles, which the weight gradients and the fold launches would read
+  if (gout_ld < n_last || (params && (!A_in || !part || !colsum_ws)) || (m_dev && (params || fold_skip)) ||
+      (Wb_head ? n_keep <= 0 || n_keep > layers[0].k : n_keep != layers[0].k))
+    return SR_EINVAL;
   int Kd = pad_to(n_last, 32);
   void* D = D0;
   void* Dn = D1;
-  int rc = sr_tc_pack_rows(gout, M, n_last, n_last, D, nullptr, s);
+  int rc = sr_tc_pack_rows(gout, M, n_last, gout_ld, D, m_dev, s);
   if (rc) return rc;
   bool had_skip = false;
   for (int l = L - 1; l >= 0; --l) {
     const sr_tc_layer& ly = layers[l];
     const void* X = l > 0 ? acts[l - 1] : A_in;
     const int Kx = l > 0 ? pad_to(ly.k, 32) : ld;
-    if (dW[l]) {
+    if (dW && dW[l]) {
       rc = sr_tc_wgrad(D, Kd, X, Kx, M, part, dW[l], ly.n, ly.k, ly.k, s);
       if (rc) return rc;
     }
-    if (db[l]) {
+    if (db && db[l]) {
       rc = sr_tc_colsum(D, M, Kd, ch, colsum_ws, colsum_slices, s);
       if (rc) return rc;
       colsum_reduce_kernel<<<(ly.n + 127) / 128, 128, 0, s>>>(colsum_ws, colsum_slices, Kd, db[l], ly.n);
@@ -415,17 +427,19 @@ int sr_tc_mlp_backward(const sr_tc_layer* layers, int L, int64_t M, int ld, int 
       if (ly.skip && !g_skip) return SR_EINVAL;
       rc = sr_tc_linear(D, ly.Wb, ly.zero_bias, M, ly.k, Kd, n_prev, SR_ACT_NONE, ch, Dn, Kd_prev, scale, nullptr, 0, 0,
                         ly.skip ? g_skip : nullptr, ly.skip ? g_skip_ld : 0, n_prev, ly.skip ? d_in : 0,
-                        stashes ? stashes[l - 1] : nullptr, acts[l - 1], pad_to(ly.k, 32), layers[l - 1].act, scale, nullptr,
+                        stashes ? stashes[l - 1] : nullptr, acts[l - 1], pad_to(ly.k, 32), layers[l - 1].act, scale, m_dev,
                         s);
       if (rc) return rc;
       had_skip |= ly.skip != 0;
       void* t = D; D = Dn; Dn = t;
       Kd = Kd_prev;
     } else {
-      rc = sr_tc_linear(D, ly.Wb, ly.zero_bias, M, ly.k, Kd, ly.k, SR_ACT_NONE, 1, nullptr, 0, scale, nullptr, 0, 0, x0_grad,
-                        ld, 0, ly.k, nullptr, nullptr, 0, 0, 1.0f, nullptr, s);
+      rc = sr_tc_linear(D, Wb_head ? Wb_head : ly.Wb, ly.zero_bias, M, n_keep, Kd, n_keep, SR_ACT_NONE, 1, nullptr, 0,
+                        scale, nullptr, 0, 0, x0_grad, ld, 0, n_keep, nullptr, nullptr, 0, 0, 1.0f, m_dev, s);
       if (rc) return rc;
-      if (ly.k < ld) zero_cols_kernel<<<sr_grid_for(M * (ld - ly.k), 256, 4), 256, 0, s>>>(x0_grad, ld, M, ly.k, ld);
+      if (!fold_skip) break;
+      if (n_keep < ld)
+        zero_cols_kernel<<<sr_grid_for(M * (ld - n_keep), 256, 4), 256, 0, s>>>(x0_grad, ld, M, n_keep, ld);
       if (had_skip)
         add_cols_kernel<<<sr_grid_for(M * d_in, 256, 4), 256, 0, s>>>(x0_grad, ld, g_skip, g_skip_ld, M, d_in);
     }

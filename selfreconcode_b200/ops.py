@@ -1094,6 +1094,24 @@ def _tc_mlp(lib, tcn, x0, ch, out, A_in=None, acts=None, m_dev=None):
     LAUNCHES += L      # check() counted one; the call is 1 + L launches
 
 
+def _tc_mlp_backward(lib, tcn, cot, bufs, acts, P, m_dev, g_out, g_skip, n_keep):
+    """Cotangent rows `cot` [P][>= n_last] of the net outputs -> d/d(embedded input) in g_out (first n_keep columns),
+    the skip layer's part in g_skip.  acts = the forward sweep's tiles; bufs = a pair of staging tile buffers the layers
+    alternate between; m_dev: optional device-side row count."""
+    global LAUNCHES
+    L = len(tcn.layers)
+    acts_c = (C.c_void_p * max(L - 1, 1))(*[a.data_ptr() for a in acts])
+    head = tcn.wb_head(n_keep) if n_keep < tcn.layers[0]["k"] else None
+    rc = lib.sr_tc_mlp_backward(tcn.c_layers, L, P, g_out.shape[1], tcn.fused.desc.d_in, 1, _p(cot), cot.shape[1],
+                                None, acts_c, None, _p(bufs[0]), _p(bufs[1]), None, None, 0, None, None, _p(g_out),
+                                _p(g_skip), g_skip.shape[1], _p(head), n_keep, 0, _p(m_dev), _stream())
+    if rc == _lib.SR_EUNSUPPORTED:
+        raise RuntimeError("selfrecon_b200: the tensor-core reverse sweep takes at most one skip layer; "
+                           "use the fp32 engine (trace mode 'reverse', shade_geometry) for this network")
+    check(rc, "tc_mlp_backward")
+    LAUNCHES += L      # check() counted one; the call is 1 + L launches
+
+
 def tc_mlp_forward(fused, pts, ch=1, conds=None, batch_inds=None, pts_per_frame=0, n_out=None):
     """Whole MLP on the tensor-core engine: embed -> pack -> one wgmma launch per layer.
     Returns out fp32 [P*ch, n_out] (last-layer outputs; tangent rows hold d out / d p_t)."""
@@ -1153,37 +1171,6 @@ class _TcTraceBuffers:
             self.A_in_d = u8(lib.sr_tc_act_bytes(P, 256))
             self.A_d = [u8(lib.sr_tc_act_bytes(P, widest)) for _ in range(2)]
             self.gskip_d = f32(P, 64)
-
-
-def _tc_backward_sweep(lib, tcn, cot, bufs, acts, P, m_dev, g_out, g_skip, n_keep):
-    """cotangent rows `cot` [P][32] of the net outputs -> d/d(embedded input) in g_out [P][ld]
-    (first n_keep columns), skip-connection part in g_skip.  acts = the forward sweep's tiles; bufs = a pair of
-    staging tile buffers the layers alternate between."""
-    if sum(ly["skip"] for ly in tcn.layers) > 1:
-        # each skip layer's launch stores its input-gradient part into g_skip, so a second one would overwrite the first
-        raise RuntimeError("selfrecon_b200: the tensor-core reverse sweep takes at most one skip layer; "
-                           "use the fp32 engine (trace mode 'reverse', shade_geometry) for this network")
-    d_in = tcn.fused.desc.d_in
-    cur, nxt = bufs
-    check(lib.sr_tc_pack_rows(_p(cot), P, 32, 32, _p(cur), _p(m_dev), _stream()), "tc_pack_rows")
-    K = 32
-    for l in range(len(tcn.layers) - 1, -1, -1):
-        ly = tcn.layers[l]
-        scale = 0.7071067811865476 if ly["skip"] else 1.0
-        if l > 0:
-            n_prev = tcn.layers[l - 1]["n"]
-            Kn = _pad(n_prev, 32)
-            gk = g_skip if ly["skip"] else None
-            check(lib.sr_tc_linear(_p(cur), _p(ly["Wb"]), _p(ly["zero_bias"]), P, ly["k"], K, n_prev, 0, 1, _p(nxt),
-                                   Kn, scale, None, 0, 0, _p(gk), gk.shape[1] if gk is not None else 0, n_prev,
-                                   d_in if gk is not None else 0, None, _p(acts[l - 1]), _pad(ly["k"], 32),
-                                   tcn.layers[l - 1]["act"], scale, _p(m_dev), _stream()), "tc_linear")
-            cur, nxt, K = nxt, cur, Kn
-        else:
-            Wb, N = (tcn.wb_head(n_keep), n_keep) if n_keep < ly["k"] else (ly["Wb"], ly["k"])
-            check(lib.sr_tc_linear(_p(cur), _p(Wb), _p(ly["zero_bias"]), P, N, K, N, 0, 1, None, 0,
-                                   scale, None, 0, 0, _p(g_out), g_out.shape[1], 0, n_keep, None, None, 0, 0, 1.0,
-                                   _p(m_dev), _stream()), "tc_linear")
 
 
 class _TcTraceCtx:
@@ -1279,12 +1266,12 @@ def _tc_trace_body(lib, G, sdf_net, def_net, ts, td, tp, P, times, condlen, has_
         if dual:
             side.wait_stream(main)
             with torch.cuda.stream(side):
-                _tc_backward_sweep(lib, td, B.cot_d, B.A_d, B.acts_d, P, m_dev, B.gd, B.gskip_d, 3 + 6 * dd.multires)
-        _tc_backward_sweep(lib, ts, B.cot_s, B.A, B.acts_s, P, m_dev, B.gs, B.gskip, ds.d_in)
+                _tc_mlp_backward(lib, td, B.cot_d, B.A_d, B.acts_d, P, m_dev, B.gd, B.gskip_d, 3 + 6 * dd.multires)
+        _tc_mlp_backward(lib, ts, B.cot_s, B.A, B.acts_s, P, m_dev, B.gs, B.gskip, ds.d_in)
         if dual:
             main.wait_stream(side)
         elif def_net is not None:
-            _tc_backward_sweep(lib, td, B.cot_d, B.A, B.acts_d, P, m_dev, B.gd, B.gskip, 3 + 6 * dd.multires)
+            _tc_mlp_backward(lib, td, B.cot_d, B.A, B.acts_d, P, m_dev, B.gd, B.gskip, 3 + 6 * dd.multires)
         has_skip = any(l["skip"] for l in ts.layers)
         check(lib.sr_tc_trace_update(_p(idx), _p(m_dev), P, _p(pts), _p(B.gs), B.gs.shape[1],
                                      _p(B.gskip) if has_skip else None, B.gskip.shape[1],
@@ -1435,7 +1422,7 @@ def _sdf_grad_tc(lib, sdf_full, pts, P):
     check(lib.sr_tc_embed(_p(pts), P, d.multires, pw, 1, None, None, 0, 0, _p(emb), B.ld, None, None, _stream()),
           "tc_embed")
     _tc_mlp(lib, ts, emb, 1, out, B.A_in, B.acts)
-    _tc_backward_sweep(lib, tv, B.cot, B.A, B.acts, P, None, g_out, B.g_skip, d.d_in)
+    _tc_mlp_backward(lib, tv, B.cot, B.A, B.acts, P, None, g_out, B.g_skip, d.d_in)
     has_skip = any(l["skip"] for l in ts.layers)
     check(lib.sr_tc_embed_backward(_p(pts), P, d.multires, pw, 1, _p(g_out), B.ld, _p(B.g_skip) if has_skip else None,
                                    B.ld, _p(grad), _stream()), "tc_embed_backward")

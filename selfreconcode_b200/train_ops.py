@@ -45,14 +45,6 @@ class MlpConfig:
         self.packs = packs
 
 
-def _pack_weights(lib, w):
-    w = w.contiguous()
-    n, k = w.shape
-    buf = torch.empty((lib.sr_tc_weight_bytes(n, k),), dtype=torch.uint8, device=w.device)
-    check(lib.sr_tc_pack_weights(_p(w), n, k, w.shape[1], _p(buf), _stream()), "tc_pack_weights")
-    return buf
-
-
 class _Workspace:
     """Scratch shared by backward passes on one (device, stream): wgrad partials, column-sum partials."""
     _pool = {}
@@ -97,7 +89,7 @@ class _Arena:
         return self.base + off
 
 
-def _layer_array(lib, cfg, Ws, bs, dev):
+def _layer_array(cfg, Ws, bs, dev):
     """ctypes array of sr_tc_layer (+ the tensors that must stay alive): the module's persistent packs when given,
     else packed here from the weight tensors."""
     L = len(Ws)
@@ -109,8 +101,8 @@ def _layer_array(lib, cfg, Ws, bs, dev):
         if pk is not None and (pk["n"], pk["k"]) == (n, k):
             W, Wb, bias, zb = pk["W"], pk["Wb"], pk["bias"], pk["zero_bias"]
         else:
-            W = _pack_weights(lib, Ws[i])
-            Wb = _pack_weights(lib, Ws[i].t().contiguous())          # [k rows, n cols]
+            W = ops.tc_pack_weights(Ws[i])
+            Wb = ops.tc_pack_weights(Ws[i].t())          # [k rows, n cols]
             bias = torch.zeros((_pad(n, 256),), dtype=torch.float32, device=dev)
             if bs[i] is not None:
                 bias[:n] = bs[i].detach().float()
@@ -136,7 +128,7 @@ class TcMlpFunction(torch.autograd.Function):
         bs = [wb[2 * i + 1] for i in range(L)]
         ch = cfg.ch
         with torch.cuda.device(dev):
-            layers, keep = _layer_array(lib, cfg, Ws, bs, dev)
+            layers, keep = _layer_array(cfg, Ws, bs, dev)
             ar = _Arena(dev)
             _, o_in = ar.add(lib.sr_tc_act_bytes(M, ld))
             o_act, o_st = [], []
@@ -199,11 +191,12 @@ class TcMlpFunction(torch.autograd.Function):
             db_c = (C.c_void_p * L)(*[dbs[l].data_ptr() if want_b[l] else None for l in range(L)])
             x0_grad = torch.empty((M, ld), dtype=torch.float32, device=dev) if need_x0 else None
             fa = ctx.arena
-            check(lib.sr_tc_mlp_backward(ctx.layers, L, M, ld, cfg.d_in, ch, _p(g), C.c_void_p(fa.ptr(ctx.o_in)), ctx.acts_c,
-                                         ctx.stashes_c, C.c_void_p(ar.ptr(o_d0)), C.c_void_p(ar.ptr(o_d1)),
+            check(lib.sr_tc_mlp_backward(ctx.layers, L, M, ld, cfg.d_in, ch, _p(g), shapes[-1][0],
+                                         C.c_void_p(fa.ptr(ctx.o_in)), ctx.acts_c, ctx.stashes_c,
+                                         C.c_void_p(ar.ptr(o_d0)), C.c_void_p(ar.ptr(o_d1)),
                                          C.c_void_p(ar.ptr(o_part)), C.c_void_p(ar.ptr(o_cs)), COLSUM_SLICES, dW_c, db_c,
                                          _p(x0_grad), C.c_void_p(ar.ptr(o_gs)) if o_gs is not None else None, gs_ld,
-                                         _stream()), "tc_mlp_backward")
+                                         None, shapes[0][1], 1, None, _stream()), "tc_mlp_backward")
             ops.LAUNCHES += 5 * L
         grads = []
         for l in range(L):

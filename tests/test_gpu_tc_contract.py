@@ -9,7 +9,8 @@ window.
   * invariants that need no tolerance: row independence, m_dev, determinism;
   * sr_tc_wgrad at its split and accumulator-flush edges, sr_tc_colsum at ragged row counts;
   * negative controls: every bar rejects a reference that lacks the term it guards;
-  * argument checks; skip layers whose input n + d_in crosses a multiple of 256, layer by layer and end to end.
+  * argument checks; skip layers whose input n + d_in crosses a multiple of 256, layer by layer and end to end;
+  * sr_tc_mlp_backward's value-only reverse sweep, bit for bit against the same chain of raw sr_tc_linear launches.
 
 Every bar is norm-wise (max |err| / max |ref|, tests/helpers.norm_err) unless it says otherwise; every measured error is
 printed next to its bar.
@@ -506,9 +507,137 @@ def test_tc_linear_rejects_invalid_arguments(cuda_dev):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# end to end through TcMlpFunction
+# sr_tc_mlp_backward's value-only reverse sweep (the tracer's and shading's) against the same chain as raw launches
 # ---------------------------------------------------------------------------------------------------------------------
 F, T_ = False, True
+SWEEPS = {
+    # the SDF's value-only view: one skip layer (input 473 + 39), a device-side row count inside a row tile
+    "sdf_skip_m_dev": dict(dims=[512, 512, 473, 512, 512, 1], acts=[SP] * 5 + [NONE], skips=[F, F, F, T_, F, F],
+                           d_in=39, ld=64, P=5000, m_dev=3001, n_keep=39),
+    # the translator: the input layer's launch keeps the 39 positional-encoding columns of its 167 inputs
+    "translator_head": dict(dims=[256, 256, 256, 256, 3], acts=[RELU] * 4 + [NONE], skips=[F] * 5, d_in=167, ld=192,
+                            P=4100, m_dev=None, n_keep=39),
+}
+
+
+def _sweep_net(lib, dev, c, seed):
+    """Packs, a sr_tc_layer array and the kept tiles of one ch = 1 forward sweep of a seeded network."""
+    from test_gpu_train import _case
+    from selfreconcode_b200._lib import TcLayer
+    x0, Ws, bs, _ = _case(dev, 1, c["dims"], c["acts"], c["skips"], c["d_in"], c["ld"], c["P"], seed)
+    Ls = []
+    arr = (TcLayer * len(Ws))()
+    for i, (W, b) in enumerate(zip(Ws, bs)):
+        n, k = W.shape
+        W = W.to(dev)
+        bias = torch.zeros(_pad(n, 256), device=dev)
+        bias[:n] = b.to(dev)
+        Ls.append(dict(W=W, Wp=pack_weights(lib, W), Wb=pack_weights(lib, W.t().contiguous()), bias=bias,
+                       zb=torch.zeros(_pad(k, 256), device=dev), n=n, k=k, act=c["acts"][i], skip=c["skips"][i]))
+        a = arr[i]
+        a.W, a.Wb, a.bias, a.zero_bias = (Ls[i][t].data_ptr() for t in ("Wp", "Wb", "bias", "zb"))
+        a.n, a.k, a.act, a.skip = n, k, Ls[i]["act"], int(Ls[i]["skip"])
+    M = c["P"]
+    x0 = x0.to(dev)
+    A_in = torch.empty(lib.sr_tc_act_bytes(M, c["ld"]), dtype=torch.uint8, device=dev)
+    acts = [torch.empty(lib.sr_tc_act_bytes(M, _pad(L["k"], 32)), dtype=torch.uint8, device=dev) for L in Ls[1:]]
+    acts_c = (C.c_void_p * len(acts))(*[t.data_ptr() for t in acts])
+    out = torch.empty(M, Ls[-1]["n"], device=dev)
+    assert lib.sr_tc_mlp_forward(arr, len(Ls), _p(x0), M, c["ld"], c["d_in"], 1, _p(A_in), acts_c, None, _p(out), None,
+                                 0, _stream()) == 0
+    return Ls, arr, acts, acts_c
+
+
+def _reverse_by_layers(lib, Ls, cot, bufs, acts, M, m_dev, g_out, g_skip, n_keep, head, d_in):
+    """The value-only reverse sweep as one sr_tc_linear launch per layer: pack the cotangent's 32 columns, then from the
+    last layer down a reverse launch into the other staging buffer (act' from the previous layer's kept tiles, the skip
+    scale as scale and mul_scale, a skip layer's input-gradient part into g_skip), and the input layer into g_out."""
+    cur, nxt = bufs
+    assert lib.sr_tc_pack_rows(_p(cot), M, 32, 32, _p(cur), _p(m_dev), _stream()) == 0
+    K = 32
+    for l in range(len(Ls) - 1, -1, -1):
+        L = Ls[l]
+        scale = INV_SQRT2 if L["skip"] else 1.0
+        if l > 0:
+            n_prev, Kn = Ls[l - 1]["n"], _pad(Ls[l - 1]["n"], 32)
+            gk = g_skip if L["skip"] else None
+            assert linear(lib, cur, L["Wb"], L["zb"], M, L["k"], K, n_prev, NONE, 1, A_next=nxt, K_next=Kn, scale=scale,
+                          out=gk, out_col0=n_prev, out_n=d_in if gk is not None else 0, mul_tiles=acts[l - 1],
+                          mul_K=_pad(L["k"], 32), mul_act=Ls[l - 1]["act"], mul_scale=scale, m_dev=m_dev) == 0
+            cur, nxt, K = nxt, cur, Kn
+        else:
+            Wb, N = (head, n_keep) if head is not None else (L["Wb"], L["k"])
+            assert linear(lib, cur, Wb, L["zb"], M, N, K, N, NONE, 1, scale=scale, out=g_out, out_n=n_keep,
+                          m_dev=m_dev) == 0
+
+
+@pytest.mark.parametrize("name", list(SWEEPS))
+def test_mlp_backward_value_sweep_matches_layer_launches(cuda_dev, name):
+    lib, c = _lib(), SWEEPS[name]
+    Ls, arr, acts, acts_c = _sweep_net(lib, cuda_dev, c, seed=23)
+    M, n_last, n_keep = c["P"], Ls[-1]["n"], c["n_keep"]
+    head = pack_weights(lib, Ls[0]["W"].t()[:n_keep].contiguous()) if n_keep < Ls[0]["k"] else None
+    cot = torch.zeros(M, 32, device=cuda_dev)          # sr_tc_trace_mid's rows: zero past the net's outputs
+    cot[:, :n_last] = torch.randn(M, n_last, generator=torch.Generator().manual_seed(5)).to(cuda_dev)
+    m = c["m_dev"]
+    md = torch.tensor([m], dtype=torch.int32, device=cuda_dev) if m is not None else None
+    widest = max(_pad(L["n"], 32) for L in Ls[:-1])
+    res = []
+    for chain in (True, False):
+        bufs = [sentinel(lib.sr_tc_act_bytes(M, widest), cuda_dev) for _ in range(2)]
+        g_out, g_skip = sentinel_f32(M, 64, cuda_dev), sentinel_f32(M, 64, cuda_dev)
+        if chain:
+            rc = lib.sr_tc_mlp_backward(arr, len(Ls), M, 64, c["d_in"], 1, _p(cot), 32, None, acts_c, None, _p(bufs[0]),
+                                        _p(bufs[1]), None, None, 0, None, None, _p(g_out), _p(g_skip), 64, _p(head),
+                                        n_keep, 0, _p(md), _stream())
+            assert rc == 0
+        else:
+            _reverse_by_layers(lib, Ls, cot, bufs, acts, M, md, g_out, g_skip, n_keep, head, c["d_in"])
+        torch.cuda.synchronize()
+        res.append((g_out, g_skip))
+    (g1, s1), (g2, s2) = res
+    assert torch.equal(bits(g1), bits(g2)) and torch.equal(bits(s1), bits(s2))
+    rows = m if m is not None else M
+    assert (bits(g1[:rows, :n_keep]) != SENT).any(dim=1).all() and (bits(g1[:, n_keep:]) == SENT).all()
+    assert (bits(g1[rows:]) == SENT).all() and (bits(s1[rows:]) == SENT).all(), "rows past m_dev are left alone"
+    if any(L["skip"] for L in Ls):
+        assert (bits(s1[:rows, :c["d_in"]]) != SENT).any(dim=1).all()
+    else:
+        assert (bits(s1) == SENT).all()
+
+
+def test_mlp_backward_rejects_two_skip_layers_and_invalid_arguments(cuda_dev):
+    from selfreconcode_b200._lib import SR_EINVAL, SR_EUNSUPPORTED
+    lib = _lib()
+    c = dict(SWEEPS["sdf_skip_m_dev"], P=1000)
+    Ls, arr, acts, acts_c = _sweep_net(lib, cuda_dev, c, seed=24)
+    M = c["P"]
+    cot = torch.zeros(M, 32, device=cuda_dev)
+    md = torch.tensor([500], dtype=torch.int32, device=cuda_dev)
+    bufs = [sentinel(lib.sr_tc_act_bytes(M, 512), cuda_dev) for _ in range(2)]
+    g_out, g_skip = sentinel_f32(M, 64, cuda_dev), sentinel_f32(M, 64, cuda_dev)
+
+    def call(arr=arr, gout_ld=32, n_keep=39, fold_skip=0, m_dev=None, head=None):
+        return lib.sr_tc_mlp_backward(arr, len(Ls), M, 64, 39, 1, _p(cot), gout_ld, None, acts_c, None, _p(bufs[0]),
+                                      _p(bufs[1]), None, None, 0, None, None, _p(g_out), _p(g_skip), 64, _p(head),
+                                      n_keep, fold_skip, _p(m_dev), _stream())
+
+    two = type(arr)(*arr)                   # a copy of the layer array with a second skip layer (same widths)
+    two[1].skip = 1
+    assert arr[1].skip == 0
+    assert call(arr=two) == SR_EUNSUPPORTED
+    bad = {"gout_ld < n_last": dict(gout_ld=0), "n_keep != k without a head": dict(n_keep=32),
+           "head wider than k": dict(n_keep=40, head=Ls[0]["Wb"]), "m_dev with fold_skip": dict(fold_skip=1, m_dev=md)}
+    for what, kw in bad.items():
+        assert call(**kw) == SR_EINVAL, what
+    torch.cuda.synchronize()
+    for t in bufs + [g_out, g_skip]:
+        assert (bits(t) == SENT).all(), "a refused call launches nothing"
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# end to end through TcMlpFunction
+# ---------------------------------------------------------------------------------------------------------------------
 CASES = {
     # the skip layer's input is 256 + 39 = 295 columns: past the forward's last column tile, and the reverse launch's
     # width pads to 512 while the stash it reads is 256 wide.  At 2 800 rows the 256 x 256 layer's weight gradient
