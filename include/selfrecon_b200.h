@@ -485,9 +485,7 @@ int sr_weight_norm_backward(const sr_wn_layer* layers, int L, cudaStream_t s);
  * a sign (`> balance`, MCAcc/seg3d_lossless.py:333-346) or threshold (`< dthreshold`,
  * utils/FindSurfacePs.py:120-127) decision on a value inside that band is re-taken on the fp32 FFMA engine:
  * sr_band_select lists the ids with |v - center| < eps (device-side count, caller zeroes it),
- * sr_sdf_forward_indexed re-evaluates exactly those points and overwrites sdf[id].  For the tracer,
- * sr_tc_trace_mid (below) lists the rays whose convergence test could flip within (eps_f, eps_a [degrees]) and
- * sr_trace_step_rev (test-only: active_out = NULL, active_in = that list) decides them. */
+ * sr_sdf_forward_indexed re-evaluates exactly those points and overwrites sdf[id]. */
 int sr_band_select(const float* values, int64_t n, float center, float eps, int32_t* list,
                    int32_t* counter, cudaStream_t s);
 int sr_sdf_forward_indexed(const sr_mlp_desc* net, const float* pts, int64_t P, const int32_t* index,
@@ -505,14 +503,11 @@ int sr_sdf_forward_small(const sr_mlp_desc* net, const float* pts, int64_t P, co
 int sr_tc_trace_mid(const int32_t* index, const int32_t* m_dev, int64_t P, const float* pts,
                     const float* rays, const int64_t* batch_inds, const float* f, const float* off,
                     const sr_lbs_params* lbs, const sr_trace_params* tp, int do_update,
-                    uint8_t* converged, float* dsdf, float* ddef, int ld, float* aux,
-                    int32_t* recheck /* [P] or NULL */, int32_t* recheck_count, float eps_f, float eps_a,
-                    cudaStream_t s);
+                    uint8_t* converged, float* dsdf, float* ddef, int ld, float* aux, cudaStream_t s);
 int sr_tc_trace_update(const int32_t* index, const int32_t* m_dev, int64_t P, float* pts,
                        const float* gs, int gs_ld, const float* gskip, int gk_ld, const float* gd,
                        int gd_ld, const float* aux, int mr_s, const float* pw_s, int mr_d,
-                       const float* pw_d, int32_t* active_out, int32_t* counter_out,
-                       const uint8_t* converged /* or NULL */, cudaStream_t s);
+                       const float* pw_d, int32_t* active_out, int32_t* counter_out, cudaStream_t s);
 
 /* Shading on the tensor-core engine: sr_tc_shade_point turns grad f [P,3] (the SDF's reverse sweep
  * through sr_tc_embed_backward) and the 4-rows-per-point translator outputs (offset / d offset) into

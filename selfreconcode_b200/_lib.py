@@ -120,10 +120,9 @@ SIGNATURES = {
     "sr_tc_linear": (C.c_int, [c_f, c_f, c_f, i64, i32, i32, i32, i32, i32, c_f, i32, f32, c_f, i32,
                                i32, c_f, i32, i32, i32, c_f, c_f, i32, i32, f32, c_f, stream_t]),
     "sr_tc_trace_mid": (C.c_int, [c_f, c_f, i64, c_f, c_f, c_f, c_f, c_f, C.POINTER(LbsParams),
-                                  C.POINTER(TraceParams), i32, c_f, c_f, c_f, i32, c_f, c_f, c_f, f32, f32,
-                                  stream_t]),
+                                  C.POINTER(TraceParams), i32, c_f, c_f, c_f, i32, c_f, stream_t]),
     "sr_tc_trace_update": (C.c_int, [c_f, c_f, i64, c_f, c_f, i32, c_f, i32, c_f, i32, c_f, i32,
-                                     C.POINTER(f32), i32, C.POINTER(f32), c_f, c_f, c_f, stream_t]),
+                                     C.POINTER(f32), i32, C.POINTER(f32), c_f, c_f, stream_t]),
     "sr_raster_mesh": (C.c_int, [c_f, c_f, i64, i64, i64, i32, i32, c_f, c_f, c_f, c_f, stream_t]),
     "sr_mesh_vertex_normals": (C.c_int, [c_f, c_f, c_f, c_f, i64, i64, i64, c_f, stream_t]),
     "sr_shade_phong": (C.c_int, [c_f, c_f, c_f, c_f, i64, i64, i64, c_f, c_f, i32, i32, c_f, c_f,

@@ -9,6 +9,7 @@
 // stride-9 per-thread accesses of the reference into fully coalesced 128-bit global
 // transactions; the grid is a multiple of the SM count with a grid-stride loop.
 #include "common.cuh"
+#include "trace_rules.cuh"
 
 namespace {
 
@@ -33,13 +34,6 @@ __device__ __forceinline__ void store_tile(T* __restrict__ g, const T* s, int64_
   for (int i = tid; i < cnt * 9; i += kThreads) dst[i] = s[i];
 }
 
-// 2x2 minor of rows (r0,r1) x cols (c0,c1):  a*d - b*c written exactly as the reference
-// writes its cofactors so that nvcc's FMA contraction produces the same rounding.
-template <typename T>
-__device__ __forceinline__ T minor2(const T* m, int r0, int c0, int r1, int c1) {
-  return m[3 * r0 + c0] * m[3 * r1 + c1] - m[3 * r0 + c1] * m[3 * r1 + c0];
-}
-
 template <typename T>
 __global__ void __launch_bounds__(kThreads)
 minv3x3_kernel(const T* __restrict__ ms, T* __restrict__ invs, uint8_t* __restrict__ checks,
@@ -55,23 +49,11 @@ minv3x3_kernel(const T* __restrict__ ms, T* __restrict__ invs, uint8_t* __restri
       T m[9];
 #pragma unroll
       for (int i = 0; i < 9; ++i) m[i] = sm[tid * 9 + i];  // stride 9: conflict free (9 odd)
-      // cofactors cof[r][c] (sign folded in by swapping the minor's columns)
-      T c00 = minor2(m, 1, 1, 2, 2);
-      T c01 = -m[3] * m[8] + m[5] * m[6];
-      T c02 = minor2(m, 1, 0, 2, 1);
-      T c10 = -m[1] * m[8] + m[2] * m[7];
-      T c11 = minor2(m, 0, 0, 2, 2);
-      T c12 = -m[0] * m[7] + m[1] * m[6];
-      T c20 = minor2(m, 0, 1, 1, 2);
-      T c21 = -m[0] * m[5] + m[2] * m[3];
-      T c22 = minor2(m, 0, 0, 1, 1);
-      T det = m[0] * c00 + m[1] * c01 + m[2] * c02;
-      bool ok = !(fabs((double)det) < 0.0001);
-      T o[9];
+      T c[9], det, o[9];
+      const bool ok = minv3x3_cofactors(m, c, det);
       if (ok) {
-        o[0] = c00 / det; o[1] = c10 / det; o[2] = c20 / det;
-        o[3] = c01 / det; o[4] = c11 / det; o[5] = c21 / det;
-        o[6] = c02 / det; o[7] = c12 / det; o[8] = c22 / det;
+#pragma unroll
+        for (int i = 0; i < 9; ++i) o[i] = c[3 * (i % 3) + i / 3] / det;  // o[r][k] = c[k][r] / det
       } else {
 #pragma unroll
         for (int i = 0; i < 9; ++i) o[i] = T(0);

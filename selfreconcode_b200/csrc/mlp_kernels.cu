@@ -9,6 +9,7 @@
 // doubling as the TMA producer, ~221 KB dynamic shared memory, one CTA per SM.
 #include "mlp_core.cuh"
 #include "lbs.cuh"
+#include "trace_rules.cuh"
 
 using namespace srmlp;
 
@@ -445,40 +446,19 @@ trace_kernel(const __grid_constant__ TraceArgs args) {
       const int gp = __float_as_int(a[AUX_GP]);
       if (gp >= 0) {
         const float f = a[AUX_F];
-        const float vx = args.rays[(size_t)gp * 3], vy = args.rays[(size_t)gp * 3 + 1],
-                    vz = args.rays[(size_t)gp * 3 + 2];
-        const float ux = a[AUX_D] - args.tp.cam_pos[0], uy = a[AUX_D + 1] - args.tp.cam_pos[1],
-                    uz = a[AUX_D + 2] - args.tp.cam_pos[2];
-        // up = u x v
-        const float cx = uy * vz - uz * vy, cy = uz * vx - ux * vz, cz = ux * vy - uy * vx;
-        const float n_up = sqrtf(cx * cx + cy * cy + cz * cz);
-        const float n_u = sqrtf(ux * ux + uy * uy + uz * uz);
-        const float sang = n_up / n_u;
-        const float ang = asinf(sang) * 180.0f / 3.14159265358979323846f;
-        const bool done = (fabsf(f) < args.tp.dthreshold) && (ang < args.tp.athreshold);
-        if (done) {
+        const RayTest r = ray_test(f, a + AUX_D, args.rays + (size_t)gp * 3, args.tp);
+        if (r.done) {
           args.converged[gp] = 1;
         } else if (args.do_update) {
-          // loss = w1 |f| + w2 |n_up / n_u| ;  g = d loss / d p
-          const float loss = args.tp.w1 * fabsf(f) + args.tp.w2 * fabsf(sang);
-          float q[3] = {0.f, 0.f, 0.f};  // d loss2 / d u
-          if (n_up > 0.f) {
-            // d n_up / d u = (v x up) / n_up
-            const float wx = vy * cz - vz * cy, wy = vz * cx - vx * cz, wz = vx * cy - vy * cx;
-            const float i1 = 1.0f / (n_up * n_u), i2 = n_up / (n_u * n_u * n_u);
-            q[0] = wx * i1 - ux * i2; q[1] = wy * i1 - uy * i2; q[2] = wz * i1 - uz * i2;
-          }
-          const float sgn = f > 0.f ? 1.f : (f < 0.f ? -1.f : 0.f);
+          // g = d loss / d p = w1 sign(f) grad f + w2 J^T q
+          float u[3];
+          const float loss = ray_loss(r, f, a + AUX_J, args.tp, u);
+          const float cot_f = sdf_cotangent(f, args.tp);
           float g[3];
 #pragma unroll
-          for (int j = 0; j < 3; ++j)
-            g[j] = args.tp.w1 * sgn * a[AUX_GF + j] +
-                   args.tp.w2 * (a[AUX_J + j] * q[0] + a[AUX_J + 3 + j] * q[1] + a[AUX_J + 6 + j] * q[2]);
-          const float t = -loss / (g[0] * g[0] + g[1] * g[1] + g[2] * g[2]);
-#pragma unroll
-          for (int j = 0; j < 3; ++j) args.pts[(size_t)gp * 3 + j] = a[AUX_P + j] + t * g[j];
-          const int slot = atomicAdd(&args.counters[args.iter + 1], 1);
-          args.active_out[slot] = gp;
+          for (int j = 0; j < 3; ++j) g[j] = cot_f * a[AUX_GF + j] + u[j];
+          newton_step(args.pts + (size_t)gp * 3, a + AUX_P, g, loss, &args.counters[args.iter + 1], args.active_out,
+                      gp);
         }
       }
     }
@@ -547,32 +527,13 @@ trace_rev_kernel(const __grid_constant__ TraceRevArgs ra) {
       int state = 0;  // 0: padding / done, 1: needs update
       if (gp >= 0) {
         const float f = a[AUX_F];
-        const float vx = args.rays[(size_t)gp * 3], vy = args.rays[(size_t)gp * 3 + 1],
-                    vz = args.rays[(size_t)gp * 3 + 2];
-        const float ux = a[AUX_D] - args.tp.cam_pos[0], uy = a[AUX_D + 1] - args.tp.cam_pos[1],
-                    uz = a[AUX_D + 2] - args.tp.cam_pos[2];
-        const float cx = uy * vz - uz * vy, cy = uz * vx - ux * vz, cz = ux * vy - uy * vx;
-        const float n_up = sqrtf(cx * cx + cy * cy + cz * cz);
-        const float n_u = sqrtf(ux * ux + uy * uy + uz * uz);
-        const float sang = n_up / n_u;
-        const float ang = asinf(sang) * 180.0f / 3.14159265358979323846f;
-        const bool done = (fabsf(f) < args.tp.dthreshold) && (ang < args.tp.athreshold);
-        if (done) {
+        const RayTest r = ray_test(f, a + AUX_D, args.rays + (size_t)gp * 3, args.tp);
+        if (r.done) {
           args.converged[gp] = 1;
         } else if (args.do_update) {
           state = 1;
-          loss = args.tp.w1 * fabsf(f) + args.tp.w2 * fabsf(sang);
-          float q[3] = {0.f, 0.f, 0.f};
-          if (n_up > 0.f) {
-            const float wx = vy * cz - vz * cy, wy = vz * cx - vx * cz, wz = vx * cy - vy * cx;
-            const float i1 = 1.0f / (n_up * n_u), i2 = n_up / (n_u * n_u * n_u);
-            q[0] = wx * i1 - ux * i2; q[1] = wy * i1 - uy * i2; q[2] = wz * i1 - uz * i2;
-          }
-          cot_f = args.tp.w1 * (f > 0.f ? 1.f : (f < 0.f ? -1.f : 0.f));
-          // u = w2 * M^T q : cotangent of p' = p + offset (also the direct dD/dp term)
-#pragma unroll
-          for (int j = 0; j < 3; ++j)
-            u[j] = args.tp.w2 * (a[AUX_J + j] * q[0] + a[AUX_J + 3 + j] * q[1] + a[AUX_J + 6 + j] * q[2]);
+          loss = ray_loss(r, f, a + AUX_J, args.tp, u);
+          cot_f = sdf_cotangent(f, args.tp);
         }
       }
       a[AUX_F] = cot_f;                 // slots reused: cotangent of f
@@ -621,11 +582,8 @@ trace_rev_kernel(const __grid_constant__ TraceRevArgs ra) {
             embed_backward(c.s.at, threadIdx.x, x, args.dnet.multires, args.dnet.pe_w, gd);
             g[0] += gd[0]; g[1] += gd[1]; g[2] += gd[2];
           }
-          const float t = -a[AUX_OFF] / (g[0] * g[0] + g[1] * g[1] + g[2] * g[2]);
-#pragma unroll
-          for (int j = 0; j < 3; ++j) args.pts[(size_t)gp * 3 + j] = x[j] + t * g[j];
-          const int slot = atomicAdd(&args.counters[args.iter + 1], 1);
-          args.active_out[slot] = gp;
+          newton_step(args.pts + (size_t)gp * 3, x, g, a[AUX_OFF], &args.counters[args.iter + 1], args.active_out,
+                      gp);
         }
       }
     }
@@ -694,34 +652,8 @@ shade_kernel(const __grid_constant__ ShadeArgs args) {
       const float* a = c.aux + threadIdx.x * kAuxStride;
       const int gp = __float_as_int(a[AUX_GP]);
       if (gp >= 0) {
-        // n = grad f / |grad f|        (model/network.py:357-358)
-        const float gx = a[AUX_GF], gy = a[AUX_GF + 1], gz = a[AUX_GF + 2];
-        const float gn = sqrtf(gx * gx + gy * gy + gz * gz);
-        args.normals[(size_t)gp * 3] = gx / gn;
-        args.normals[(size_t)gp * 3 + 1] = gy / gn;
-        args.normals[(size_t)gp * 3 + 2] = gz / gn;
-        // cardinal ray = normalize(J^-1 v), fallback v      (utils/utils.py:155-169)
-        const float* m = a + AUX_J;
-        const float c00 = m[4] * m[8] - m[5] * m[7], c01 = -m[3] * m[8] + m[5] * m[6],
-                    c02 = m[3] * m[7] - m[4] * m[6];
-        const float c10 = -m[1] * m[8] + m[2] * m[7], c11 = m[0] * m[8] - m[2] * m[6],
-                    c12 = -m[0] * m[7] + m[1] * m[6];
-        const float c20 = m[1] * m[5] - m[2] * m[4], c21 = -m[0] * m[5] + m[2] * m[3],
-                    c22 = m[0] * m[4] - m[1] * m[3];
-        const float det = m[0] * c00 + m[1] * c01 + m[2] * c02;
-        const bool ok = !(fabs((double)det) < 0.0001);
-        const float vx = args.rays[(size_t)gp * 3], vy = args.rays[(size_t)gp * 3 + 1],
-                    vz = args.rays[(size_t)gp * 3 + 2];
-        float rx = vx, ry = vy, rz = vz;
-        if (ok) {
-          rx = (c00 / det) * vx + (c10 / det) * vy + (c20 / det) * vz;
-          ry = (c01 / det) * vx + (c11 / det) * vy + (c21 / det) * vz;
-          rz = (c02 / det) * vx + (c12 / det) * vy + (c22 / det) * vz;
-        }
-        const float rn = sqrtf(rx * rx + ry * ry + rz * rz);
-        args.crays[(size_t)gp * 3] = rx / rn;
-        args.crays[(size_t)gp * 3 + 1] = ry / rn;
-        args.crays[(size_t)gp * 3 + 2] = rz / rn;
+        const bool ok = shade_point(a + AUX_GF, a + AUX_J, args.rays + (size_t)gp * 3, args.normals + (size_t)gp * 3,
+                                    args.crays + (size_t)gp * 3);
         if (args.dpos) {
 #pragma unroll
           for (int j = 0; j < 3; ++j) args.dpos[(size_t)gp * 3 + j] = a[AUX_D + j];

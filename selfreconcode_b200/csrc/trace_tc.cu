@@ -7,6 +7,7 @@
 //                damped Newton step p <- p - loss/|g|^2 g, device-side append to the next list
 #include "common.cuh"
 #include "lbs.cuh"
+#include "trace_rules.cuh"
 
 namespace {
 
@@ -28,12 +29,6 @@ struct MidArgs {
   float* ddef;             // [M][ld] cotangent rows for the translator backward sweep (cols 0..2)
   int ld;
   float* aux;              // [M][8]: loss, state, u[3]
-  // borderline decisions: the tensor-core engine's f / D(p) carry up to ~2.4e-5 / ~1e-5 of error, so a
-  // ray whose test could flip inside (eps_f, eps_a) is NOT decided here: it is appended to `recheck`
-  // and re-tested by the fp32 FFMA engine (sr_trace_step_rev, test-only) before the update kernel runs.
-  int* recheck;            // [P] or null (then the test below is final)
-  int* recheck_count;
-  float eps_f, eps_a;
 };
 
 __global__ void __launch_bounds__(256) trace_mid_kernel(const __grid_constant__ MidArgs a) {
@@ -63,35 +58,14 @@ __global__ void __launch_bounds__(256) trace_mid_kernel(const __grid_constant__ 
     }
     if (lane == 0) {
       const float f = a.f[i];
-      const float vx = a.rays[gp * 3], vy = a.rays[gp * 3 + 1], vz = a.rays[gp * 3 + 2];
-      const float ux = d[0] - a.tp.cam_pos[0], uy = d[1] - a.tp.cam_pos[1], uz = d[2] - a.tp.cam_pos[2];
-      const float cx = uy * vz - uz * vy, cy = uz * vx - ux * vz, cz = ux * vy - uy * vx;
-      const float n_up = sqrtf(cx * cx + cy * cy + cz * cz);
-      const float n_u = sqrtf(ux * ux + uy * uy + uz * uz);
-      const float sang = n_up / n_u;
-      const float ang = asinf(sang) * 180.0f / 3.14159265358979323846f;
-      bool done = (fabsf(f) < a.tp.dthreshold) && (ang < a.tp.athreshold);
-      if (a.recheck != nullptr) {
-        const bool maybe = (fabsf(f) < a.tp.dthreshold + a.eps_f) && (ang < a.tp.athreshold + a.eps_a);
-        const bool sure = (fabsf(f) < a.tp.dthreshold - a.eps_f) && (ang < a.tp.athreshold - a.eps_a);
-        if (maybe && !sure) a.recheck[atomicAdd(a.recheck_count, 1)] = (int)gp;
-        done = sure;
-      }
+      const RayTest r = ray_test(f, d, a.rays + gp * 3, a.tp);
       float u[3] = {0.f, 0.f, 0.f}, loss = 0.f;
       int state = 0;
-      if (done) {
+      if (r.done) {
         a.converged[gp] = 1;
       } else if (a.do_update) {
         state = 1;
-        loss = a.tp.w1 * fabsf(f) + a.tp.w2 * fabsf(sang);
-        float q[3] = {0.f, 0.f, 0.f};
-        if (n_up > 0.f) {
-          const float wx = vy * cz - vz * cy, wy = vz * cx - vx * cz, wz = vx * cy - vy * cx;
-          const float i1 = 1.0f / (n_up * n_u), i2 = n_up / (n_u * n_u * n_u);
-          q[0] = wx * i1 - ux * i2; q[1] = wy * i1 - uy * i2; q[2] = wz * i1 - uz * i2;
-        }
-#pragma unroll
-        for (int j = 0; j < 3; ++j) u[j] = a.tp.w2 * (Mm[j] * q[0] + Mm[3 + j] * q[1] + Mm[6 + j] * q[2]);
+        loss = ray_loss(r, f, Mm, a.tp, u);
       }
       float* ax = a.aux + i * 8;
       ax[0] = loss; ax[1] = __int_as_float(state); ax[2] = u[0]; ax[3] = u[1]; ax[4] = u[2];
@@ -103,7 +77,7 @@ __global__ void __launch_bounds__(256) trace_mid_kernel(const __grid_constant__ 
       float vs = 0.f, vd = 0.f;
       if (k == 0) {
         const float f = a.f[i];
-        vs = (__float_as_int(ax[1]) == 1) ? a.tp.w1 * (f > 0.f ? 1.f : (f < 0.f ? -1.f : 0.f)) : 0.f;
+        vs = (__float_as_int(ax[1]) == 1) ? sdf_cotangent(f, a.tp) : 0.f;
       }
       if (k < 3) vd = ax[2 + k];
       a.dsdf[i * a.ld + k] = vs;
@@ -130,7 +104,6 @@ struct UpdArgs {
   float pw_d[16];
   int* active_out;
   int* counter_out;
-  const unsigned char* converged;   // rays the fp32 re-test declared done after trace_mid (or null)
 };
 
 __device__ __forceinline__ void pe_chain(const float* g, const float* gk, const float x[3], int multires,
@@ -159,16 +132,11 @@ __global__ void __launch_bounds__(256) trace_update_kernel(const __grid_constant
     const float* ax = a.aux + i * 8;
     if (__float_as_int(ax[1]) != 1) continue;
     const long long gp = a.index ? (long long)a.index[i] : i;
-    if (a.converged != nullptr && a.converged[gp]) continue;
     const float x[3] = {a.pts[gp * 3], a.pts[gp * 3 + 1], a.pts[gp * 3 + 2]};
     float g[3] = {ax[2], ax[3], ax[4]};  // direct term u (d p' / d p = I + d off / d p)
     pe_chain(a.gs + i * a.gs_ld, a.gskip ? a.gskip + i * a.gk_ld : nullptr, x, a.mr_s, a.pw_s, g);
     if (a.gd) pe_chain(a.gd + i * a.gd_ld, nullptr, x, a.mr_d, a.pw_d, g);
-    const float t = -ax[0] / (g[0] * g[0] + g[1] * g[1] + g[2] * g[2]);
-#pragma unroll
-    for (int j = 0; j < 3; ++j) a.pts[gp * 3 + j] = x[j] + t * g[j];
-    const int slot = atomicAdd(a.counter_out, 1);
-    a.active_out[slot] = (int)gp;
+    newton_step(a.pts + gp * 3, x, g, ax[0], a.counter_out, a.active_out, (int)gp);
   }
 }
 
@@ -221,23 +189,7 @@ __global__ void __launch_bounds__(256) shade_point_kernel(const __grid_constant_
       for (int r = 0; r < 3; ++r)
 #pragma unroll
         for (int c = 0; c < 3; ++c) m[3 * r + c] = Mm[3 * r] * Q[c] + Mm[3 * r + 1] * Q[3 + c] + Mm[3 * r + 2] * Q[6 + c];
-      const float gx = a.grad[i * 3], gy = a.grad[i * 3 + 1], gz = a.grad[i * 3 + 2];
-      const float gn = sqrtf(gx * gx + gy * gy + gz * gz);
-      a.normals[i * 3] = gx / gn; a.normals[i * 3 + 1] = gy / gn; a.normals[i * 3 + 2] = gz / gn;
-      const float c00 = m[4] * m[8] - m[5] * m[7], c01 = -m[3] * m[8] + m[5] * m[6], c02 = m[3] * m[7] - m[4] * m[6];
-      const float c10 = -m[1] * m[8] + m[2] * m[7], c11 = m[0] * m[8] - m[2] * m[6], c12 = -m[0] * m[7] + m[1] * m[6];
-      const float c20 = m[1] * m[5] - m[2] * m[4], c21 = -m[0] * m[5] + m[2] * m[3], c22 = m[0] * m[4] - m[1] * m[3];
-      const float det = m[0] * c00 + m[1] * c01 + m[2] * c02;
-      const bool ok = !(fabs((double)det) < 0.0001);
-      const float vx = a.rays[i * 3], vy = a.rays[i * 3 + 1], vz = a.rays[i * 3 + 2];
-      float rx = vx, ry = vy, rz = vz;
-      if (ok) {
-        rx = (c00 / det) * vx + (c10 / det) * vy + (c20 / det) * vz;
-        ry = (c01 / det) * vx + (c11 / det) * vy + (c21 / det) * vz;
-        rz = (c02 / det) * vx + (c12 / det) * vy + (c22 / det) * vz;
-      }
-      const float rn = sqrtf(rx * rx + ry * ry + rz * rz);
-      a.crays[i * 3] = rx / rn; a.crays[i * 3 + 1] = ry / rn; a.crays[i * 3 + 2] = rz / rn;
+      const bool ok = shade_point(a.grad + i * 3, m, a.rays + i * 3, a.normals + i * 3, a.crays + i * 3);
       if (a.dpos) { a.dpos[i * 3] = d[0]; a.dpos[i * 3 + 1] = d[1]; a.dpos[i * 3 + 2] = d[2]; }
       if (a.inv_ok) a.inv_ok[i] = ok ? 1 : 0;
     }
@@ -316,17 +268,15 @@ int sr_tc_render_embed(int64_t P, const float* pts, const float* views, const fl
 int sr_tc_trace_mid(const int32_t* index, const int32_t* m_dev, int64_t P, const float* pts,
                     const float* rays, const int64_t* batch_inds, const float* f, const float* off,
                     const sr_lbs_params* lbs, const sr_trace_params* tp, int do_update,
-                    uint8_t* converged, float* dsdf, float* ddef, int ld, float* aux,
-                    int32_t* recheck, int32_t* recheck_count, float eps_f, float eps_a, cudaStream_t s) {
+                    uint8_t* converged, float* dsdf, float* ddef, int ld, float* aux, cudaStream_t s) {
   if (!pts || !rays || !f || !tp || !converged || !dsdf || !aux || P <= 0 || ld < 8) return SR_EINVAL;
-  if ((recheck != nullptr) != (recheck_count != nullptr) || eps_f < 0.f || eps_a < 0.f) return SR_EINVAL;
   MidArgs a;
   a.index = index; a.m_dev = m_dev; a.P = P; a.pts = pts; a.rays = rays;
   a.batch_inds = (const long long*)batch_inds; a.f = f; a.off = off;
   a.has_lbs = lbs ? 1 : 0;
   if (lbs) a.lbs = *lbs;
   a.tp = *tp; a.do_update = do_update; a.converged = converged; a.dsdf = dsdf; a.ddef = ddef; a.ld = ld;
-  a.aux = aux; a.recheck = recheck; a.recheck_count = recheck_count; a.eps_f = eps_f; a.eps_a = eps_a;
+  a.aux = aux;
   trace_mid_kernel<<<sr_grid_for(P * 32, 256, 8), 256, 0, s>>>(a);
   return sr_launch_status();
 }
@@ -334,14 +284,13 @@ int sr_tc_trace_mid(const int32_t* index, const int32_t* m_dev, int64_t P, const
 int sr_tc_trace_update(const int32_t* index, const int32_t* m_dev, int64_t P, float* pts,
                        const float* gs, int gs_ld, const float* gskip, int gk_ld, const float* gd,
                        int gd_ld, const float* aux, int mr_s, const float* pw_s, int mr_d,
-                       const float* pw_d, int32_t* active_out, int32_t* counter_out,
-                       const uint8_t* converged, cudaStream_t s) {
+                       const float* pw_d, int32_t* active_out, int32_t* counter_out, cudaStream_t s) {
   if (!pts || !gs || !aux || !active_out || !counter_out || !pw_s || P <= 0) return SR_EINVAL;
   UpdArgs a;
   a.index = index; a.m_dev = m_dev; a.P = P; a.pts = pts; a.gs = gs; a.gs_ld = gs_ld; a.gskip = gskip;
   a.gk_ld = gk_ld; a.gd = gd; a.gd_ld = gd_ld; a.aux = aux; a.mr_s = mr_s; a.mr_d = mr_d;
   for (int i = 0; i < 16; ++i) { a.pw_s[i] = i < mr_s ? pw_s[i] : 0.f; a.pw_d[i] = (pw_d && i < mr_d) ? pw_d[i] : 0.f; }
-  a.active_out = active_out; a.counter_out = counter_out; a.converged = converged;
+  a.active_out = active_out; a.counter_out = counter_out;
   trace_update_kernel<<<sr_grid_for(P, 256, 8), 256, 0, s>>>(a);
   return sr_launch_status();
 }

@@ -23,15 +23,12 @@ TC_ENABLED = _os.environ.get("SELFRECON_B200_TC", "1") != "0"
 # 2048: below it a tensor-core trace is launch bound and the fp32 engine (one persistent kernel) is the faster choice
 TC_MIN_POINTS = int(_os.environ.get("SELFRECON_B200_TC_MIN_POINTS", "2048"))
 
-# Borderline decisions on tensor-core values are re-taken on the fp32 FFMA engine (DESIGN.md section 4):
-# TC_EPS_F bounds the engine's absolute error on an SDF value (split-BF16 with fp32 accumulation, csrc/tc_gemm.cu),
-# TC_EPS_A (degrees) the error of the ray/point angle that follows from D(p)'s.
+# The tensor-core engine's error bounds (DESIGN.md section 4): TC_EPS_F bounds its absolute error on an SDF value
+# (split-BF16 with fp32 accumulation, csrc/tc_gemm.cu), and sign decisions inside it are re-taken on the fp32 FFMA
+# engine (sdf_refine_band); TC_EPS_A (degrees) is the error of the ray/point angle that follows from D(p)'s.
 TC_EPS_F = float(_os.environ.get("SELFRECON_B200_TC_EPS_F", "4e-5"))
 TC_EPS_A = float(_os.environ.get("SELFRECON_B200_TC_EPS_A", "1e-3"))
 TC_REFINE = _os.environ.get("SELFRECON_B200_TC_REFINE", "1") != "0"
-# The tracer's in-loop fp32 re-test costs one latency-bound FFMA launch per iteration and cannot remove the dominant source of per-ray divergence (sign(f) in the update when |f| is below the
-# engine's error, DESIGN.md section 4): off by default, kept for experiments.
-TC_REFINE_TRACE = _os.environ.get("SELFRECON_B200_TC_REFINE_TRACE", "0") != "0"
 TC_DUAL_STREAM = _os.environ.get("SELFRECON_B200_TC_DUAL_STREAM", "1") != "0"
 
 import itertools as _it
@@ -837,30 +834,29 @@ def trace_surface_points(sdf_net, def_net, lbs, cam_pos, rays, init_pts, batch_i
     Nothing syncs the host.  mode: "tc" = dense layers on the tensor-core engine (wgmma split-BF16,
     reverse-mode sweeps), "reverse" / "forward" = fused fp32 FFMA engine (times+1 launches of one
     persistent kernel), "auto" = "tc" for large ray sets, "reverse" otherwise."""
-    if mode == "auto":
-        mode = "tc" if (TC_ENABLED and init_pts.shape[0] >= TC_MIN_POINTS) else "reverse"
-    if mode == "tc":
-        return trace_surface_points_tc(sdf_net, def_net, lbs, cam_pos, rays, init_pts, batch_inds, conds,
-                                       dthreshold, athreshold, w1, w2, times, return_counters)
     _need_cuda(rays, init_pts)
     dev = init_pts.device
     P = init_pts.shape[0]
+    if P == 0:
+        pts, conv = init_pts.detach().float().clone(), torch.zeros((0,), dtype=torch.bool, device=dev)
+        return (pts, conv, torch.zeros((times + 3,), dtype=torch.int32, device=dev)) if return_counters \
+            else (pts, conv)
+    tp = TraceParams()
+    tp.cam_pos[:] = _host_floats(cam_pos)[:3]
+    tp.dthreshold, tp.athreshold, tp.w1, tp.w2 = float(dthreshold), float(athreshold), float(w1), float(w2)
+    if mode == "auto":
+        mode = "tc" if (TC_ENABLED and P >= TC_MIN_POINTS) else "reverse"
+    if mode == "tc":
+        return _trace_surface_points_tc(sdf_net, def_net, lbs, tp, rays, init_pts, batch_inds, conds, times,
+                                        return_counters)
     pts = init_pts.detach().contiguous().float().clone()
     rays = rays.detach().contiguous().float()
     bi = batch_inds.contiguous().to(torch.int64) if batch_inds is not None else None
     conds = conds.detach().contiguous().float() if conds is not None else None
     condlen = conds.shape[-1] if conds is not None else 0
     conv = torch.zeros((P,), dtype=torch.bool, device=dev)
-    if P == 0:
-        return (pts, conv, torch.zeros((times + 3,), dtype=torch.int32, device=dev)) if return_counters \
-            else (pts, conv)
     lists = [torch.empty((P,), dtype=torch.int32, device=dev) for _ in range(2)]
     counters = torch.zeros((times + 3,), dtype=torch.int32, device=dev)
-    tp = TraceParams()
-    cp = _host_floats(cam_pos)
-    for i in range(3):
-        tp.cam_pos[i] = cp[i]
-    tp.dthreshold, tp.athreshold, tp.w1, tp.w2 = float(dthreshold), float(athreshold), float(w1), float(w2)
     lib = _lib.load()
     dref = C.byref(def_net.desc) if def_net is not None else None
     with torch.cuda.device(dev):
@@ -1190,11 +1186,7 @@ class _TcTraceCtx:
         self.lbsA = torch.empty((n_frames, 24, 4, 4), dtype=torch.float32, device=dev)
         self.lbsT = torch.empty((n_frames, 3), dtype=torch.float32, device=dev)
         self.lbs_params = LbsParams()
-        # borderline rays of each iteration, re-tested on the fp32 engine (one list, one count per iteration)
         self.side_stream = torch.cuda.Stream(device=dev)
-        self.recheck = torch.empty((P,), dtype=torch.int32, device=dev)
-        self.recheck_counts = torch.empty((times + 1,), dtype=torch.int32, device=dev)
-        self.rev_scratch = _trace_scratch(dev)
         self.graph = None
         self.sig = None
         self.calls = 0
@@ -1216,10 +1208,6 @@ def _tc_trace_body(lib, G, sdf_net, def_net, ts, td, tp, P, times, condlen, has_
     conv.zero_()
     counters.zero_()
     counters[0:1].fill_(P)
-    refine = TC_REFINE_TRACE
-    if refine:
-        G.recheck_counts.zero_()
-    dref = C.byref(def_net.desc) if def_net is not None else None
     for it in range(times + 1):
         idx = lists[(it + 1) & 1] if it > 0 else None
         a_out = lists[it & 1] if it < times else None
@@ -1249,17 +1237,8 @@ def _tc_trace_body(lib, G, sdf_net, def_net, ts, td, tp, P, times, condlen, has_
         check(lib.sr_tc_trace_mid(_p(idx), _p(m_dev), P, _p(pts), _p(rays), _p(bi), _p(B.f),
                                   _p(B.off) if def_net is not None else None, lbs_ref, C.byref(tp),
                                   1 if a_out is not None else 0, _p(conv), _p(B.cot_s),
-                                  _p(B.cot_d) if def_net is not None else None, 32, _p(B.aux),
-                                  _p(G.recheck) if refine else None,
-                                  _p(G.recheck_counts[it:it + 1]) if refine else None,
-                                  TC_EPS_F if refine else 0.0, TC_EPS_A if refine else 0.0, _stream()),
+                                  _p(B.cot_d) if def_net is not None else None, 32, _p(B.aux), _stream()),
               "tc_trace_mid")
-        if refine:
-            # fp32 re-test of the borderline rays (test-only launch: no update, marks converged[])
-            check(lib.sr_trace_step_rev(C.byref(sdf_net.desc), dref, lbs_ref, C.byref(tp), _p(pts), _p(rays),
-                                        _p(bi), _p(conds), condlen, P, _p(G.recheck), None,
-                                        _p(G.recheck_counts), it, _p(conv), _p(G.rev_scratch), _stream()),
-                  "trace_step_rev")
         if a_out is None:
             break
         # ---- reverse sweeps + update
@@ -1278,41 +1257,30 @@ def _tc_trace_body(lib, G, sdf_net, def_net, ts, td, tp, P, times, condlen, has_
                                      _p(B.gd) if def_net is not None else None,
                                      B.gd.shape[1] if def_net is not None else 0, _p(B.aux), ds.multires,
                                      pw_s, dd.multires if dd is not None else 0, pw_d, _p(a_out),
-                                     _p(counters[it + 1:it + 2]), _p(conv) if refine else None, _stream()),
+                                     _p(counters[it + 1:it + 2]), _stream()),
               "tc_trace_update")
 
 
-def trace_surface_points_tc(sdf_net, def_net, lbs, cam_pos, rays, init_pts, batch_inds, conds,
-                            dthreshold=5e-5, athreshold=0.02, w1=3.05, w2=1.0, times=5,
-                            return_counters=False):
-    """OptimizeSurfacePs with the dense layers on the tensor-core engine (reverse-mode sweeps).
-    Same contract as trace_surface_points.  A trace is ~35 launches per iteration, all with static
-    shapes and device-side counts, so from the second call with the same configuration (ray count,
-    networks, thresholds, PE weights) the whole trace is replayed as one CUDA graph
-    (SELFRECON_B200_GRAPHS=0 keeps it eager)."""
+def _trace_surface_points_tc(sdf_net, def_net, lbs, tp, rays, init_pts, batch_inds, conds, times, return_counters):
+    """trace_surface_points with the dense layers on the tensor-core engine (reverse-mode sweeps), for
+    P > 0 rays.  A trace is ~35 launches per iteration, all with static shapes and device-side counts, so
+    from the second call with the same configuration (ray count, networks, thresholds, PE weights) the
+    whole trace is replayed as one CUDA graph (SELFRECON_B200_GRAPHS=0 keeps it eager)."""
     global LAUNCHES
-    _need_cuda(rays, init_pts)
     dev = init_pts.device
     P = init_pts.shape[0]
-    if P == 0:
-        pts = init_pts.detach().float().clone()
-        conv = torch.zeros((0,), dtype=torch.bool, device=dev)
-        return (pts, conv, torch.zeros((times + 3,), dtype=torch.int32, device=dev)) if return_counters \
-            else (pts, conv)
     lib = _lib.load()
     condlen = conds.shape[-1] if conds is not None else 0
     n_frames = lbs.A.shape[0] if lbs is not None else (conds.shape[0] if conds is not None else 1)
-    cp = _host_floats(cam_pos)
     ds, dd = sdf_net.desc, (def_net.desc if def_net is not None else None)
     # buffers depend on shapes only; the captured graph also on everything a launch bakes in
     key = (dev.index, P, tuple(ds.layer[i].n for i in range(ds.n_layers)),
            tuple(dd.layer[i].n for i in range(dd.n_layers)) if dd is not None else (), n_frames, condlen,
            conds.shape[0] if conds is not None else 0, times)
     sig = (sdf_net.uid, def_net.uid if def_net is not None else -1,
-           lbs.ws_cl.data_ptr() if lbs is not None else 0, cp, float(dthreshold), float(athreshold),
-           float(w1), float(w2), tuple(ds.pe_w[i] for i in range(ds.multires)),
-           tuple(dd.pe_w[i] for i in range(dd.multires)) if dd is not None else (),
-           TC_REFINE_TRACE, TC_EPS_F, TC_EPS_A, TC_DUAL_STREAM)
+           lbs.ws_cl.data_ptr() if lbs is not None else 0, tuple(tp.cam_pos), tp.dthreshold, tp.athreshold,
+           tp.w1, tp.w2, tuple(ds.pe_w[i] for i in range(ds.multires)),
+           tuple(dd.pe_w[i] for i in range(dd.multires)) if dd is not None else (), TC_DUAL_STREAM)
     G = _tc_trace_ctx.get(key)
     if G is None:
         if len(_tc_trace_ctx) >= 4:
@@ -1322,10 +1290,6 @@ def trace_surface_points_tc(sdf_net, def_net, lbs, cam_pos, rays, init_pts, batc
     if G.sig != sig:          # new weights / thresholds: the old graph is stale, buffers are not
         G.sig, G.graph, G.calls = sig, None, 0
     ts, td = tc_net(sdf_net), (tc_net(def_net) if def_net is not None else None)
-    tp = TraceParams()
-    for i in range(3):
-        tp.cam_pos[i] = cp[i]
-    tp.dthreshold, tp.athreshold, tp.w1, tp.w2 = float(dthreshold), float(athreshold), float(w1), float(w2)
     with torch.cuda.device(dev):
         G.pts.copy_(init_pts.detach().reshape(P, 3))
         G.rays.copy_(rays.detach().reshape(P, 3))
