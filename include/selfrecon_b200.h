@@ -360,6 +360,41 @@ int sr_points_silhouette_backward(const float* pts_screen, const float* grad_mas
                                   const float* prod, const int32_t* zeros, int64_t N, int64_t V, int H, int W,
                                   float radius, float* grad_pts, cudaStream_t s);
 
+/* Template mesh regularisers of OptimNetwork.computeTmpPcLoss (model/network.py:655-670): pytorch3d 0.4.0's
+ * mesh_laplacian_smoothing(method='uniform'), mesh_edge_loss(target_length=0.) and mesh_normal_consistency of one mesh,
+ * verts [V,3] float, faces [F,3] int64, V <= 2^31.
+ * Topology, once per face table (Meshes._compute_packed):
+ *   sr_mesh_reg_edge_keys: keys [3F]; entry 3f+k = the edge opposite corner k of face f as the hash V*min + max of its
+ *     two vertex ids, or -1 when either id is outside [0, V).  The caller sorts the keys stably (keeping perm).
+ *   sr_mesh_reg_edge_runs: over the n sorted keys: head[i] = 1 where a run of equal keys (one unique edge) starts, else
+ *     0; npairs[i] = the run's pair count at a head ((m-1)^2 - (m-2) for a run of m >= 2 entries), else 0.
+ *   sr_mesh_reg_topology: head_cum / pair_cum = inclusive prefix sums of head / npairs, E = head_cum[3F-1],
+ *     P = pair_cum[3F-1].  Writes edges [E,2] (a <= b, ascending hash), face_to_edge [F,3], dir_keys [2E] (V*a+b and
+ *     V*b+a of each edge: sorted by the caller into the directed neighbour CSR) and pairs [P,4] = (a, b, o_i, o_j), the
+ *     opposite corners of pytorch3d's literal list [e[i], e[j]] for i in range(m-1) for j in range(1, m) if i != j over
+ *     each edge's entries e in ascending (face, corner) order.
+ * sr_mesh_reg_forward: out [3] = (sum_i |(L v)_i| / V, sum_e |v_a - v_b|^2 / E, sum_p (1 - cos(n_i, -n_j)) / P or 0),
+ *   fp64 inside.  nbr_off [V+1] / nbr = each vertex's directed neighbours (a self-edge twice), ascending; L v =
+ *   mean of the neighbours - v (-v without neighbours).  n = (v_b - v_a) x (v_o - v_a), exactly 0 with no gradient
+ *   when o = a, o = b or a = b; cos = w12 / sqrt(max(w1 w2, 1e-16)).  Workspace for the backward: u [V,3] = (L v)_i / |(L v)_i| (0 at a zero norm), dn [P,6] = d(1 - cos)/dn_i,
+ *   d/dn_j; partials = 3 * SR_MESH_REG_BLOCKS doubles.  Two launches: block partials, then a fixed-order sum.
+ * sr_mesh_reg_backward: grad_verts [V,3] for the cotangent grad_out [3] (device), one thread per vertex gathering over
+ *   its neighbours and its (pair, role) entries vp_off [V+1] / vp_ent (= 4 p + role, role = the vertex's column of
+ *   pairs), in CSR order.
+ * pairs, dn and vp_ent may be NULL when P = 0.  No atomics: bit-identical reruns. */
+#define SR_MESH_REG_BLOCKS 528
+int sr_mesh_reg_edge_keys(const int64_t* faces, int64_t F, int64_t V, int64_t* keys, cudaStream_t s);
+int sr_mesh_reg_edge_runs(const int64_t* sorted_keys, int64_t n, int64_t* head, int64_t* npairs, cudaStream_t s);
+int sr_mesh_reg_topology(const int64_t* faces, const int64_t* sorted_keys, const int64_t* perm, const int64_t* head_cum,
+                         const int64_t* pair_cum, int64_t F, int64_t V, int64_t E, int64_t P, int64_t* edges,
+                         int64_t* face_to_edge, int64_t* dir_keys, int64_t* pairs, cudaStream_t s);
+int sr_mesh_reg_forward(const float* verts, int64_t V, int64_t E, int64_t P, const int64_t* edges,
+                        const int64_t* nbr_off, const int64_t* nbr, const int64_t* pairs, double* u, double* dn,
+                        double* partials, float* out, cudaStream_t s);
+int sr_mesh_reg_backward(const float* verts, int64_t V, int64_t E, int64_t P, const int64_t* nbr_off,
+                         const int64_t* nbr, const int64_t* pairs, const int64_t* vp_off, const int64_t* vp_ent,
+                         const double* u, const double* dn, const float* grad_out, float* grad_verts, cudaStream_t s);
+
 /* Texture atlas of the reconstruction (texture_mesh_extract.py:57-144: VideoAvatar's Isomapper aggregation), over the
  * T atlas texels a UV face covers (the UV raster: sr_raster_mesh on the atlas), S <= SR_TEXTURE_MAX_SLOTS slots each.
  * Slots are slot-major: slot_rgb [S][3][T] (colour in [0,1], planar), slot_alpha [S][T] (c0 = cos(max_angle) when

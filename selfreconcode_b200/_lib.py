@@ -132,6 +132,11 @@ SIGNATURES = {
     "sr_points_silhouette_forward": (C.c_int, [c_f, c_f, c_f, i64, i64, i32, i32, f32, i32, c_f, c_f, c_f, c_f,
                                                stream_t]),
     "sr_points_silhouette_backward": (C.c_int, [c_f, c_f, c_f, c_f, c_f, i64, i64, i32, i32, f32, c_f, stream_t]),
+    "sr_mesh_reg_edge_keys": (C.c_int, [c_f, i64, i64, c_f, stream_t]),
+    "sr_mesh_reg_edge_runs": (C.c_int, [c_f, i64, c_f, c_f, stream_t]),
+    "sr_mesh_reg_topology": (C.c_int, [c_f, c_f, c_f, c_f, c_f, i64, i64, i64, i64, c_f, c_f, c_f, c_f, stream_t]),
+    "sr_mesh_reg_forward": (C.c_int, [c_f, i64, i64, i64, c_f, c_f, c_f, c_f, c_f, c_f, c_f, c_f, stream_t]),
+    "sr_mesh_reg_backward": (C.c_int, [c_f, i64, i64, i64, c_f, c_f, c_f, c_f, c_f, c_f, c_f, c_f, c_f, stream_t]),
     "sr_texture_accumulate": (C.c_int, [i64, i32, c_f, c_f, c_f, c_f, i64, i64, c_f, c_f, c_f, i32, i32, i32, c_f, c_f,
                                         c_f, c_f, c_f, stream_t]),
     "sr_texture_finish": (C.c_int, [i64, i32, c_f, c_f, c_f, c_f, f32, i32, c_f, c_f, c_f, c_f, stream_t]),

@@ -21,6 +21,7 @@ import torch.nn as nn
 import utils
 from FastMinv import Fast3x3Minv
 import MCGpu
+from selfreconcode_b200 import ops
 from .CameraMine import RectifiedPerspectiveCameras, PointsRendererWithFrags
 
 
@@ -88,6 +89,7 @@ class OptimNetwork(nn.Module):
         self.sdfShrinkRadius = 0.0
         self.info = {}
         self.TmpPs = None
+        self.mesh_reg_topo = None  # ops.MeshRegTopology of Tmpfs, built when a mesh regulariser weight is positive
         self.raster_seed = None   # callable(frame_ids, TmpVs, Tmpfs, defconds, ratio) -> seed dict
 
     # ---- differentiable value-only evaluations (tensor-core training engine when the modules are the stock ones)
@@ -472,6 +474,7 @@ class OptimNetwork(nn.Module):
             self.TmpVs.requires_grad = True
             self.TmpOptimizer = torch.optim.SGD([self.TmpVs], lr=0.05, momentum=0.9)
             self.TmpVid, self.TmpFid = vertex_face_pairs(self.Tmpfs, self.TmpVs.shape[0])
+            self.mesh_reg_topo = None
             self.root = root
         poses, trans, d_cond, _ = self.dataset.get_grad_parameters(frame_ids, device)
         defconds = [d_cond, [poses, trans]]
@@ -539,18 +542,28 @@ class OptimNetwork(nn.Module):
         self.info['pc_loss']['mask_loss'] = mask_loss.item()
         loss = mask_loss * (conf.get_float('pc_weight.mask_weight') if 'pc_weight.mask_weight' in conf else 1.)
         has_pc = 'pc_weight' in conf
-        tmpMesh = None
-        for key, tag, fn in (('laplacian_weight', 'lap_loss', lambda P, m: P.mesh_laplacian_smoothing(m, method='uniform')),
-                             ('edge_weight', 'edge_loss', lambda P, m: P.mesh_edge_loss(m, target_length=0.)),
-                             ('norm_weight', 'norm_loss', lambda P, m: P.mesh_normal_consistency(m))):
+        tmpMesh = regs = None
+        for i, (key, tag, fn) in enumerate((
+                ('laplacian_weight', 'lap_loss', lambda P, m: P.mesh_laplacian_smoothing(m, method='uniform')),
+                ('edge_weight', 'edge_loss', lambda P, m: P.mesh_edge_loss(m, target_length=0.)),
+                ('norm_weight', 'norm_loss', lambda P, m: P.mesh_normal_consistency(m)))):
             w = conf.get_float('pc_weight.' + key) if (has_pc and ('pc_weight.' + key) in conf) else -1.
-            if w > 0.:
-                P = _p3d()      # pytorch3d's mesh regularisers (third party, outside the hot path)
+            if w <= 0.:
+                continue
+            if torch.is_tensor(defMeshes):
+                # the silhouette ran on tensors: all three terms from one device evaluation (csrc/mesh_reg.cu)
+                if regs is None:
+                    if self.mesh_reg_topo is None:
+                        self.mesh_reg_topo = ops.mesh_reg_topology(self.Tmpfs, self.TmpVs.shape[0])
+                    regs = ops.mesh_regularizers(self.TmpVs, self.mesh_reg_topo)
+                term = w * regs[i]
+            else:
+                P = _p3d()      # pytorch3d's mesh regularisers on its own containers
                 if tmpMesh is None:
                     tmpMesh = P.Meshes(verts=[self.TmpVs], faces=[self.Tmpfs])
                 term = w * fn(P, tmpMesh)
-                loss = loss + term
-                self.info['pc_loss'][tag] = term.item() / w
+            loss = loss + term
+            self.info['pc_loss'][tag] = term.item() / w
         cw = conf.get_float('pc_weight.def_consistent.weight') if 'pc_weight.def_consistent' in conf else -1.
         if cw > 0.:
             rigid = self.deformer.defs[1](self.TmpVs.view(1, -1, 3).expand(N, -1, 3), defconds[1])

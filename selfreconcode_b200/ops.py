@@ -224,6 +224,108 @@ _KERNELS_PER_CALL.update({"points_silhouette_bin": 1, "points_silhouette_forward
                           "points_silhouette_backward": 1})
 
 
+MESH_REG_BLOCKS = 528     # SR_MESH_REG_BLOCKS
+
+
+class MeshRegTopology:
+    """Device tables of one face table for mesh_regularizers (csrc/mesh_reg.cu): the unique edges [E,2] in pytorch3d's
+    order, face_to_edge [F,3], the directed neighbour CSR (nbr_off [V+1], nbr), the normal-consistency pairs [P,4] =
+    (a, b, o_i, o_j) and the vertex -> (pair, role) CSR (vp_off [V+1], vp_ent = 4 pair + role)."""
+
+    def __init__(self, V, F, E, P, edges, face_to_edge, nbr_off, nbr, pairs, vp_off, vp_ent):
+        self.V, self.F, self.E, self.P = V, F, E, P
+        self.edges, self.face_to_edge = edges, face_to_edge
+        self.nbr_off, self.nbr = nbr_off, nbr
+        self.pairs, self.vp_off, self.vp_ent = pairs, vp_off, vp_ent
+
+
+def mesh_reg_topology(faces, V):
+    """faces [F,3] int64 CUDA of a mesh with V vertices -> MeshRegTopology (pytorch3d 0.4.0 Meshes._compute_packed
+    edges and mesh_normal_consistency pairs).  Reads E and P back to the host once; a face index outside [0, V) is a
+    ValueError."""
+    _need_cuda(faces)
+    fc = faces.detach().contiguous().to(torch.int64)
+    V = int(V)
+    if fc.dim() != 2 or fc.shape[1] != 3 or fc.shape[0] == 0 or V <= 0:
+        raise ValueError("mesh_reg_topology: faces must be [F,3] with F > 0 and V > 0")
+    F = fc.shape[0]
+    dev = fc.device
+    lib = _lib.load()
+    with torch.cuda.device(dev):
+        keys = torch.empty(3 * F, dtype=torch.int64, device=dev)
+        check(lib.sr_mesh_reg_edge_keys(_p(fc), F, V, _p(keys), _stream()), "mesh_reg_edge_keys")
+        skeys, perm = torch.sort(keys, stable=True)     # unique edges ascending, (face, corner) order inside each
+        head, npairs = torch.empty_like(skeys), torch.empty_like(skeys)
+        check(lib.sr_mesh_reg_edge_runs(_p(skeys), 3 * F, _p(head), _p(npairs), _stream()), "mesh_reg_edge_runs")
+        head_cum, pair_cum = torch.cumsum(head, 0), torch.cumsum(npairs, 0)
+        bad, E, P = torch.stack([(skeys[0] < 0).long(), head_cum[-1], pair_cum[-1]]).tolist()
+        if bad:
+            raise ValueError("mesh_reg_topology: a face index is outside [0, %d)" % V)
+        edges = torch.empty((E, 2), dtype=torch.int64, device=dev)
+        f2e = torch.empty((F, 3), dtype=torch.int64, device=dev)
+        dkeys = torch.empty(2 * E, dtype=torch.int64, device=dev)
+        pairs = torch.empty((P, 4), dtype=torch.int64, device=dev)
+        check(lib.sr_mesh_reg_topology(_p(fc), _p(skeys), _p(perm), _p(head_cum), _p(pair_cum), F, V, E, P,
+                                       _p(edges), _p(f2e), _p(dkeys), _p(pairs if P else None), _stream()),
+              "mesh_reg_topology")
+        dkeys = torch.sort(dkeys).values
+        nbr_off = torch.searchsorted(dkeys, torch.arange(V + 1, dtype=torch.int64, device=dev) * V)
+        nbr = torch.remainder(dkeys, V)
+        vid, vp_ent = torch.sort(pairs.reshape(-1), stable=True)
+        vp_off = torch.searchsorted(vid, torch.arange(V + 1, dtype=torch.int64, device=dev))
+    return MeshRegTopology(V, F, E, P, edges, f2e, nbr_off, nbr, pairs, vp_off, vp_ent)
+
+
+class _MeshRegularizers(torch.autograd.Function):
+    """(laplacian, edge, normal consistency) of one mesh (csrc/mesh_reg.cu), differentiable w.r.t. the vertices."""
+
+    @staticmethod
+    def forward(ctx, verts, topo):
+        _need_cuda(verts)
+        vs = verts.detach().contiguous().float()
+        if tuple(vs.shape) != (topo.V, 3):
+            raise ValueError("mesh_regularizers: verts must be [%d,3], got %s" % (topo.V, tuple(vs.shape)))
+        dev = vs.device
+        u = torch.empty((topo.V, 3), dtype=torch.float64, device=dev)
+        dn = torch.empty((topo.P, 6), dtype=torch.float64, device=dev)
+        part = torch.empty(3 * MESH_REG_BLOCKS, dtype=torch.float64, device=dev)
+        out = torch.empty(3, dtype=torch.float32, device=dev)
+        pairs = topo.pairs if topo.P else None
+        with torch.cuda.device(dev):
+            check(_lib.load().sr_mesh_reg_forward(_p(vs), topo.V, topo.E, topo.P, _p(topo.edges), _p(topo.nbr_off),
+                                                  _p(topo.nbr), _p(pairs), _p(u), _p(dn if topo.P else None),
+                                                  _p(part), _p(out), _stream()), "mesh_reg_forward")
+        ctx.save_for_backward(vs, u, dn)
+        ctx.topo = topo
+        ctx.in_dtype = verts.dtype
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        vs, u, dn = ctx.saved_tensors
+        topo = ctx.topo
+        g = grad_out.contiguous().float()
+        out = torch.empty_like(vs)
+        has_p = topo.P > 0
+        with torch.cuda.device(vs.device):
+            check(_lib.load().sr_mesh_reg_backward(
+                _p(vs), topo.V, topo.E, topo.P, _p(topo.nbr_off), _p(topo.nbr), _p(topo.pairs if has_p else None),
+                _p(topo.vp_off), _p(topo.vp_ent if has_p else None), _p(u), _p(dn if has_p else None), _p(g),
+                _p(out), _stream()), "mesh_reg_backward")
+        return out.to(ctx.in_dtype), None
+
+
+def mesh_regularizers(verts, topo):
+    """verts [V,3] CUDA, topo = mesh_reg_topology(faces, V) -> [3] float32 = (mesh_laplacian_smoothing(method='uniform'),
+    mesh_edge_loss(target_length=0.), mesh_normal_consistency) of pytorch3d 0.4.0 on one mesh; differentiable w.r.t.
+    verts.  DESIGN.md section 3.3."""
+    return _MeshRegularizers.apply(verts, topo)
+
+
+_KERNELS_PER_CALL.update({"mesh_reg_edge_keys": 1, "mesh_reg_edge_runs": 1, "mesh_reg_topology": 1,
+                          "mesh_reg_forward": 2, "mesh_reg_backward": 1})
+
+
 TEXTURE_MAX_SLOTS = 64     # SR_TEXTURE_MAX_SLOTS
 
 
