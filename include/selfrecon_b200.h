@@ -440,6 +440,19 @@ int sr_lbsw_knn_blend(const float* verts, const float* vert_ws, int V, int C, co
 int sr_lbsw_smooth_pass(const float* src, float* dst, int C, int D, int H, int W, float cut, cudaStream_t s);
 int sr_lbsw_cut(float* field, int64_t n, float cut, cudaStream_t s);
 
+/* Device-resident frames of a sequence (dataset/dataset.py:89-102: SceneDataset.__getitem__ decoded once).  Store:
+ * img_store / normal_store uint8 [F,H,W,3] in file (BGR) order as cv2 reads it; mask_store uint32 [F,H,ceil(W/32)],
+ * bit (c & 31) of word (c >> 5) = column c has a nonzero channel, rows padded to whole words.  For n < N and
+ * f = frame_ids[n] (device int64, 0 <= f < F, checked by the caller: rows with other ids are left unwritten):
+ *   img [N,H,W,3]    = (x / 255 - 0.5) * 2                 in file order
+ *   mask [N,H,W]     = 1 where the bit is set, else 0
+ *   normal [N,H,W,3] = 2 x / 255 - 1                       channels reversed (RGB)
+ * each fp32 operation rounded on its own, so the results are bit-identical to the numpy expressions.  Any output may be
+ * NULL; the store plane an output reads must not be.  SR_EINVAL for F, H or W <= 0, N < 0 or a missing plane. */
+int sr_frames_decode(const uint8_t* img_store, const uint32_t* mask_store, const uint8_t* normal_store, int F, int H,
+                     int W, const int64_t* frame_ids, int64_t N, float* img, float* mask, float* normal,
+                     cudaStream_t s);
+
 /* Training half of the tensor-core engine (model/network.py:599-639, 774-796: loss.backward() and the parameter
  * VJPs; in a reverse launch (`mul_tiles` != NULL) `dstash` is an INPUT: the fp32 act'(z) the forward launch of the
  * previous layer wrote (leading dimension = that layer's width rounded up to 256), or NULL to recompute act' from the

@@ -144,6 +144,7 @@ SIGNATURES = {
                                     c_f, stream_t]),
     "sr_lbsw_smooth_pass": (C.c_int, [c_f, c_f, i32, i32, i32, i32, f32, stream_t]),
     "sr_lbsw_cut": (C.c_int, [c_f, i64, f32, stream_t]),
+    "sr_frames_decode": (C.c_int, [c_f, c_f, c_f, i32, i32, i32, c_f, i64, c_f, c_f, c_f, stream_t]),
     "sr_tc_wgrad_partial_bytes": (i64, [i64, i32, i32, C.POINTER(C.c_int)]),
     "sr_tc_debug_wgrad_desc_swap": (None, [i32]),
     "sr_tc_mlp_forward": (C.c_int, [C.POINTER(TcLayer), i32, c_f, i64, i32, i32, i32, c_f, C.POINTER(C.c_void_p),

@@ -11,10 +11,16 @@ Per-frame learnables (poses, trans, latent code tables) live here as leaf tensor
 reference: the DataLoader only carries images, `get_grad_parameters(ids)` slices the leaves so gradients reach
 them.  Additions for multi-GPU runs: `ShardedSampler` (one disjoint, equally long index stream per rank,
 SURVEY.md section 8e) and pinned host staging of the frame tensors.
+
+Once `getOptNet` has recorded the training device on the dataset, the loader of `getDatasetAndLoader` keeps the
+whole sequence on that device in file form (`FrameStore`: 6.125 B per pixel) and decodes each batch there
+(csrc/frames.cu), so a step reads no image file and copies no frame from the host.
 """
 import os
 import os.path as osp
 import random
+import time
+from concurrent.futures import ThreadPoolExecutor
 from glob import glob
 
 import numpy as np
@@ -85,6 +91,12 @@ class SceneDataset(torch.utils.data.Dataset):
 
     def _stage(self, t):
         return t.pin_memory() if self.pin_memory else t
+
+    def __getstate__(self):
+        # DataLoader workers receive the dataset pickled: the device frame store stays in the main process
+        state = self.__dict__.copy()
+        state.pop('_frame_store', None)
+        return state
 
     def __getitem__(self, idx):
         import cv2
@@ -204,6 +216,168 @@ class ShardedSampler(torch.utils.data.Sampler):
         return self.n
 
 
+def _normal_path(img_name):
+    return img_name.replace('/imgs/', '/normals/')[:-3] + 'png'     # as SceneDataset.__getitem__ names it
+
+
+def pack_mask(mask):
+    """Foreground of a mask as cv2 reads it ([H,W,C] or [H,W] uint8; a pixel is foreground when any channel is > 0, as
+    in SceneDataset.__getitem__) -> int32 [H, ceil(W/32)]: bit c & 31 of word c >> 5 holds column c, rows padded to
+    whole words (the mask plane of FrameStore)."""
+    fg = np.asarray(mask) > 0
+    if fg.ndim == 3:
+        fg = fg.any(-1)
+    H, W = fg.shape
+    bits = np.zeros((H, (W + 31) // 32 * 32), np.bool_)
+    bits[:, :W] = fg
+    return np.packbits(bits, axis=-1, bitorder='little').view('<u4').view(np.int32)
+
+
+class FrameStore:
+    """A sequence's frames on one device, as the files hold them: img and normal uint8 [F,H,W,3] in file (BGR) order,
+    mask bit-packed int32 [F,H,ceil(W/32)] (pack_mask).  `decode(ids)` -> the batch SceneDataset.__getitem__ and the
+    DataLoader's collate would give for the host ids, as fp32 CUDA tensors on the current stream."""
+
+    def __init__(self, img, mask, normal, W):
+        self.img, self.mask, self.normal, self.W = img, mask, normal, W
+        self.outputs = ('img', 'mask') + (('normal',) if normal is not None else ())
+
+    @staticmethod
+    def nbytes_for(F, H, W, with_normal):
+        return F * H * (3 * W * (2 if with_normal else 1) + 4 * ((W + 31) // 32))
+
+    def nbytes(self):
+        return sum(t.numel() * t.element_size() for t in (self.img, self.mask, self.normal) if t is not None)
+
+    def decode(self, ids):
+        from selfreconcode_b200 import ops
+        return ops.frames_decode(self.img, self.mask, self.normal, ids, self.W, self.outputs)
+
+
+_STAGE_BYTES = 128 << 20    # pinned staging per chunk (two chunks in flight)
+
+
+def _read_frame(paths, H, W):
+    import cv2
+    planes = []
+    for p in paths:
+        a = cv2.imread(p)
+        if a is None or a.shape != (H, W, 3):
+            raise ValueError("%s: %s, the sequence's frames are %dx%d" % (
+                p, "unreadable" if a is None else "%dx%d" % a.shape[:2], H, W))
+        planes.append(a)
+    planes[1] = pack_mask(planes[1])
+    return planes
+
+
+def _host_path_reason(dataset, device):
+    if device.type != 'cuda':
+        return "device %s is not CUDA" % device
+    if dataset.require_albedo:
+        return "albedo planes are requested"
+    n_normal = sum(osp.isfile(_normal_path(n)) for n in dataset.img_ns)
+    if 0 < n_normal < dataset.frame_num:
+        return "normals exist for %d of %d frames" % (n_normal, dataset.frame_num)
+    need = FrameStore.nbytes_for(dataset.frame_num, dataset.H, dataset.W, n_normal > 0)
+    free = torch.cuda.mem_get_info(device)[0]
+    if 2 * need > free:
+        return "the store needs %.2f GB, more than half of the %.2f GB free on %s" % (need / 1e9, free / 1e9, device)
+    return None
+
+
+def build_frame_store(dataset, device):
+    """Decodes every frame's files once on the host (a thread pool: cv2 releases the GIL), packs the masks and copies
+    the frames to `device` in chunks through pinned staging, so the host never holds the whole sequence."""
+    t0 = time.perf_counter()
+    F, H, W = dataset.frame_num, dataset.H, dataset.W
+    with_normal = osp.isfile(_normal_path(dataset.img_ns[0]))
+    shapes = [((H, W, 3), torch.uint8), ((H, (W + 31) // 32), torch.int32)] + \
+        ([((H, W, 3), torch.uint8)] if with_normal else [])
+    planes = [torch.empty((F,) + sh, dtype=dt, device=device) for sh, dt in shapes]
+    chunk = max(1, min(F, _STAGE_BYTES // (FrameStore.nbytes_for(1, H, W, with_normal))))
+    stages = [[torch.empty((chunk,) + sh, dtype=dt, pin_memory=True) for sh, dt in shapes] for _ in range(2)]
+    copied = [None, None]
+
+    def paths(i):
+        return [dataset.img_ns[i], dataset.mask_ns[i]] + ([_normal_path(dataset.img_ns[i])] if with_normal else [])
+
+    with torch.cuda.device(device), ThreadPoolExecutor(max_workers=min(16, os.cpu_count() or 1)) as pool:
+        stream = torch.cuda.current_stream()
+        for c, lo in enumerate(range(0, F, chunk)):
+            hi = min(F, lo + chunk)
+            frames = list(pool.map(lambda i: _read_frame(paths(i), H, W), range(lo, hi)))
+            st = stages[c % 2]
+            if copied[c % 2] is not None:
+                copied[c % 2].synchronize()        # this staging buffer's previous copy has left it
+            for j, fr in enumerate(frames):
+                for k, a in enumerate(fr):
+                    st[k][j].copy_(torch.from_numpy(a))
+            for k in range(len(planes)):
+                planes[k][lo:hi].copy_(st[k][:hi - lo], non_blocking=True)
+            copied[c % 2] = torch.cuda.Event()
+            copied[c % 2].record(stream)
+        stream.synchronize()
+    store = FrameStore(planes[0], planes[1], planes[2] if with_normal else None, W)
+    print("[frame store] %d frames of %dx%d%s on %s: %.2f GB, built in %.1f s" % (
+        F, H, W, " with normals" if with_normal else "", device, store.nbytes() / 1e9, time.perf_counter() - t0),
+        flush=True)
+    return store
+
+
+def frame_store(dataset):
+    """The dataset's device frame store, built at the first call after getOptNet recorded the training device
+    (`dataset.store_device`); None while the frames stay on the host, with the reason printed once."""
+    store = getattr(dataset, '_frame_store', None)
+    device = getattr(dataset, 'store_device', None)
+    if device is None or getattr(dataset, 'require_albedo', False):
+        return None
+    if store is None and getattr(dataset, '_frame_store_reason', None) is None:
+        device = torch.device(device)
+        why = _host_path_reason(dataset, device)
+        if why is not None:
+            print("[frame store] frames stay on the host: %s" % why, flush=True)
+            dataset._frame_store_reason = why
+        else:
+            store = dataset._frame_store = build_frame_store(dataset, device)
+    return store
+
+
+class FrameLoader:
+    """The loader of getDatasetAndLoader, with the DataLoader surface the drivers use: `dataset`, `batch_size`,
+    `sampler`, `num_workers`, len() (drop_last=False) and iteration -> (frame_ids int64 CPU [B], outs).
+
+    With a device frame store (frame_store), iteration runs in the main process without workers and `outs` holds
+    CUDA tensors decoded by one launch per batch; otherwise it is a torch DataLoader built with the same arguments.
+    Both paths draw the same numbers from the global RNGs in the same order, so a seeded run trains the same."""
+
+    def __init__(self, dataset, batch_size=1, sampler=None, num_workers=0):
+        self._host = torch.utils.data.DataLoader(dataset, batch_size, sampler=sampler, num_workers=num_workers)
+        self.dataset, self.batch_size, self.num_workers = dataset, batch_size, num_workers
+        self.sampler = self._host.sampler
+
+    def __len__(self):
+        return len(self._host)
+
+    def __iter__(self):
+        store = frame_store(self.dataset)
+        if store is None:
+            return iter(self._host)
+        # a DataLoader iterator draws its base seed from the global generator when it is created
+        # (_BaseDataLoaderIter), before the batch sampler first runs the sampler
+        torch.empty((), dtype=torch.int64).random_()
+        return self._batches(iter(self.sampler), store)
+
+    def _batches(self, ids, store):
+        batch = []
+        for i in ids:
+            batch.append(int(i))
+            if len(batch) == self.batch_size:
+                yield torch.tensor(batch, dtype=torch.int64), store.decode(batch)
+                batch = []
+        if batch:
+            yield torch.tensor(batch, dtype=torch.int64), store.decode(batch)
+
+
 def getDatasetAndLoader(root, conds_lens, batch_size, shuffle, num_workers, opt_pose, opt_trans, opt_camera,
                         rank=0, world=1):
     dataset = SceneDataset(root, conds_lens)
@@ -211,7 +385,7 @@ def getDatasetAndLoader(root, conds_lens, batch_size, shuffle, num_workers, opt_
     dataset.trans.requires_grad_(bool(opt_trans))
     dataset.opt_camera_params(opt_camera)
     sampler = RandomSampler(dataset, 1, shuffle) if world == 1 else ShardedSampler(dataset, rank, world, shuffle)
-    loader = torch.utils.data.DataLoader(dataset, batch_size, sampler=sampler, num_workers=num_workers)
+    loader = FrameLoader(dataset, batch_size, sampler=sampler, num_workers=num_workers)
     return dataset, loader
 
 

@@ -820,6 +820,7 @@ def getOptNet(dataset, N, bmins, bmaxs, resolutions, device, conf, use_initial_s
     optNet.register_buffer('tmpBodyNs', utils.compute_vnorms(tmpBodyVs, tmpBodyFs, vid, fid))
     optNet = optNet.to(device)
     optNet.dataset = dataset
+    dataset.store_device = device       # the loader keeps the sequence's frames on this device (dataset.frame_store)
     if dataset.poses.requires_grad or dataset.trans.requires_grad:
         optNet.dctnull = utils.DCTNullSpace(10, 30).to(device)
     return optNet, sdf_initialized

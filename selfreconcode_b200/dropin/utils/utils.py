@@ -279,9 +279,9 @@ def set_hierarchical_config(conf, name, optNet, dataloader, resolutions):
     """Switches the optimisation to hierarchy level `name` ('coarse' / 'medium' / 'fine'): new batch size,
     the level's loss / train config picked up at the next remesh, a new coarse-to-fine MC engine over the
     same box (utils/utils.py:237-256)."""
+    from dataset.dataset import FrameLoader
     bs = conf.get_int('train.' + name + '.point_render.batch_size')
-    dataloader = torch.utils.data.DataLoader(dataloader.dataset, bs, sampler=dataloader.sampler,
-                                             num_workers=dataloader.num_workers)
+    dataloader = FrameLoader(dataloader.dataset, bs, sampler=dataloader.sampler, num_workers=dataloader.num_workers)
     optNet.next_conf = conf.get_config('loss_' + name)
     optNet.next_train_conf = conf.get_config('train.' + name)
     optNet.engine = _new_engine(optNet.engine, resolutions)

@@ -417,6 +417,29 @@ def lbsw_smooth(field, times, cut=0.0):
     return src
 
 
+def frames_decode(img_store, mask_store, normal_store, frame_ids, W, outputs=("img", "mask", "normal")):
+    """One training batch from the device frame store (csrc/frames.cu): img_store / normal_store uint8 [F,H,W,3] in
+    file order (normal_store may be None), mask_store int32 [F,H,ceil(W/32)] bit-packed, frame_ids host int64 [N] (a
+    list or CPU tensor) -> {'img' [N,H,W,3], 'mask' [N,H,W], 'normal' [N,H,W,3]} fp32 on the store's device, for the
+    names in `outputs`, bit-identical to SceneDataset.__getitem__.  ValueError for an id outside [0, F)."""
+    _need_cuda(img_store, mask_store, normal_store)
+    F, H = int(mask_store.shape[0]), int(mask_store.shape[1])
+    ids = torch.as_tensor(frame_ids, dtype=torch.int64).reshape(-1)
+    if ids.is_cuda:
+        raise ValueError("frames_decode: frame ids are host integers (checked before the launch)")
+    if ids.numel() and (int(ids.min()) < 0 or int(ids.max()) >= F):
+        raise ValueError("frames_decode: frame id out of range [0, %d): %s" % (F, ids.tolist()))
+    N, dev = ids.numel(), mask_store.device
+    shapes = {"img": (N, H, W, 3), "mask": (N, H, W), "normal": (N, H, W, 3)}
+    outs = {k: torch.empty(shapes[k], dtype=torch.float32, device=dev) for k in outputs}
+    with torch.cuda.device(dev):
+        dids = ids.to(dev)
+        check(_lib.load().sr_frames_decode(_p(img_store), _p(mask_store), _p(normal_store), F, H, int(W),
+                                           _p(dids), N, _p(outs.get("img")), _p(outs.get("mask")),
+                                           _p(outs.get("normal")), _stream()), "frames_decode")
+    return outs
+
+
 def svals3x3(J, want_v=True):
     """J [n,3,3] f32 CUDA -> (singular values [n,3] descending, V [n,3,3] | None)."""
     _need_cuda(J)
@@ -906,17 +929,18 @@ _host_cache = {}
 
 def _host_floats(t):
     """Host copy of a small device tensor (camera centre), cached by (storage, version): the blocking
-    device->host read happens once per tensor value, not once per trace."""
+    device->host read happens once per tensor value, not once per trace.  Each entry holds its tensor, so
+    no other tensor can be allocated at a cached address and hit a stale entry."""
     if not t.is_cuda:
         return tuple(float(x) for x in t.detach().reshape(-1).tolist())
     key = (t.device.index, t.data_ptr(), t._version, t.numel())
-    v = _host_cache.get(key)
-    if v is None:
+    hit = _host_cache.get(key)
+    if hit is None:
         if len(_host_cache) > 64:
             _host_cache.clear()
-        v = tuple(float(x) for x in t.detach().reshape(-1).tolist())
-        _host_cache[key] = v
-    return v
+        hit = (t, tuple(float(x) for x in t.detach().reshape(-1).tolist()))
+        _host_cache[key] = hit
+    return hit[1]
 
 
 def _trace_scratch(dev):

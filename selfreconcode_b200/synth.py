@@ -313,3 +313,48 @@ class SyntheticDataset(torch.nn.Module):
     def get_camera_parameters(self, n, device):
         return (self.focals.expand(n, 2).to(device), self.pps.expand(n, 2).to(device),
                 self.Rs.expand(n, 3, 3).to(device), self.Ts.expand(n, 3).to(device), self.H, self.W)
+
+
+class _LazyFrames:
+    """Frame i of a seeded smooth sequence, made when write_sequence asks for it (a 600-frame 1080p sequence would not
+    fit in host memory as float arrays)."""
+
+    def __init__(self, F, H, W, seed, kind):
+        self.F, self.H, self.W, self.kind = F, H, W, kind
+        rs = np.random.RandomState(seed)
+        self.freq = rs.uniform(0.5, 3.0, (3, 2))
+        self.phase = rs.uniform(0, 2 * np.pi, (F, 3))
+
+    def __len__(self):
+        return self.F
+
+    def __getitem__(self, i):
+        y = np.linspace(-1, 1, self.H, dtype=np.float32)[:, None]
+        x = np.linspace(-1, 1, self.W, dtype=np.float32)[None, :]
+        if self.kind == "mask":   # an ellipse drifting with the frame index
+            cx = 0.3 * np.sin(0.2 * i)
+            return (((x - cx) / 0.45) ** 2 + (y / 0.8) ** 2 < 1).astype(np.float32)
+        ch = [np.sin(np.pi * (self.freq[c, 0] * x + self.freq[c, 1] * y) + self.phase[i, c]) for c in range(3)]
+        out = np.stack(np.broadcast_arrays(*ch), -1).astype(np.float32)
+        if self.kind == "normal":
+            out = out / np.maximum(np.linalg.norm(out, axis=-1, keepdims=True), 1e-6)
+        return 0.9 * out if self.kind == "img" else out
+
+
+def write_frame_sequence(root, F, H, W, seed=0, normals=True, image_ext=".png"):
+    """A seeded sequence of F smooth H x W frames in the on-disk layout of dataset.SceneDataset (written by
+    dataset.write_sequence; image_ext='.jpg' re-encodes the images as JPEG).  -> root"""
+    import os
+    import cv2
+    from dataset import write_sequence
+    poses, trans, _ = make_frame_params(seed, F)
+    cam = dict(fx=float(W), fy=float(W), cx=W / 2.0, cy=H / 2.0, quat=[0., 0., 0., 1.], T=[0., 0., 2.5])
+    write_sequence(root, _LazyFrames(F, H, W, seed, "img"), _LazyFrames(F, H, W, seed + 1, "mask"), poses.numpy(),
+                   trans.numpy(), np.zeros(10, np.float32), cam,
+                   normals=_LazyFrames(F, H, W, seed + 2, "normal") if normals else None)
+    if image_ext != ".png":
+        for i in range(F):
+            p = os.path.join(root, "imgs", "%06d.png" % i)
+            cv2.imwrite(p[:-4] + image_ext, cv2.imread(p))
+            os.remove(p)
+    return root
