@@ -101,6 +101,8 @@ int sr_interp2x2d_bwd_f32(const float* grad_out, float* grad_in, int bc, int h, 
  *   grad_input  : [N,C,D,H,W] contiguous, MUST be zero-filled by the caller (atomics)
  *   corner_idx (optional, may be NULL): [N,P,3] int32 = floor of the clipped
  *                 un-normalised coordinate (ix,iy,iz) -- the "skinning indices".
+ *   With C == 0 the C-sized arrays (input, output, grad_output, grad_input, gg_input,
+ *   grad_grad_output) may be NULL; corner_idx and grad_grid (zeros) are still written.
  * ------------------------------------------------------------------------------------------ */
 int sr_grid_sample3d_fwd_f32(const float* input, const int64_t* istr, const float* grid,
                              float* output, int32_t* corner_idx, int N, int C, int D, int H, int W,

@@ -2,8 +2,12 @@
 // second-order backward (SURVEY.md rows a6 / K7-K9).
 //
 // Semantics follow MCAcc/cuda/GridSamplerMineKernel.cu:160-914 of the reference:
-//   un-normalise   x -> ((x + 1.f) * W - 1.) / 2.   (float add/mul, then double, :210-212)
-//   border clip    min(W-1, max(x, 0)); gradient multiplier 0 when x<=0 or x>=W-1 (:33-61)
+//   un-normalise   x -> ((x + 1.f) * W - 1.) / 2.   (float add/mul, then double, :210-212; for
+//                  double input the product is rounded before the subtraction, never fused)
+//   border clip    min(W-1, max(x, 0)); gradient multiplier 0 when x<=0 or x>=W-1 (:33-61).
+//                  A NaN coordinate is sampled at 0 with multiplier 0, so its backward is the gradient of
+//                  what the forward computed (the reference samples it at 0 but sends its grad_input to
+//                  no voxel; the grid gradient is 0 either way)
 //   corners        floor(x) and +1; out-of-range corners are skipped (their weight is 0)
 //   forward        8 corners accumulated x-fastest, y, z with one FMA each (:285-309)
 //   backward       grad_input by atomicAdd, grad_grid scaled by W/2 and the border mask
@@ -29,11 +33,16 @@ struct Axis {
   bool in0, in1;
 };
 
+__device__ __forceinline__ float mul_rn(float a, float b) { return __fmul_rn(a, b); }
+__device__ __forceinline__ double mul_rn(double a, double b) { return __dmul_rn(a, b); }
+
 template <typename T>
 __device__ __forceinline__ Axis<T> make_axis(T g, int size) {
   Axis<T> ax;
-  // ((g + 1.f) * size - 1.) / 2.   with the reference's mixed precision
-  T prod = (g + (T)1) * (T)size;
+  // ((g + 1.f) * size - 1.) / 2.   with the reference's mixed precision.  The product is rounded to T
+  // before the subtraction in both precisions: in double the compiler would otherwise fuse
+  // `prod - 1.0` into an FMA, and x would differ by an ulp, enough to move floor(x) at a voxel face.
+  T prod = mul_rn(g + (T)1, (T)size);
   T x = (T)(((double)prod - 1.0) / 2.0);
   const T hi = (T)(size - 1);
   if (!(x > (T)0)) {  // x <= 0 (or NaN)
@@ -223,8 +232,8 @@ template <typename T>
 int fwd(const T* input, const int64_t* istr, const T* grid, T* output, int32_t* cidx, int N, int C,
         int D, int H, int W, int64_t P, cudaStream_t s) {
   if (N < 0 || C < 0 || D <= 0 || H <= 0 || W <= 0 || P < 0 || !istr) return SR_EINVAL;
-  if ((long long)N * P == 0 || C == 0) return SR_OK;
-  if (!input || !grid || !output) return SR_EINVAL;
+  if ((long long)N * P == 0 || (C == 0 && !cidx)) return SR_OK;
+  if (!grid || (C > 0 && (!input || !output))) return SR_EINVAL;
   gs3d_fwd_kernel<T><<<sr_grid_for((long long)N * P, kThreads, 16), kThreads, 0, s>>>(
       input, istr[0], istr[1], istr[2], istr[3], istr[4], grid, output, cidx, N, C, D, H, W, P);
   return sr_launch_status();
@@ -234,7 +243,7 @@ int bwd(const T* input, const int64_t* istr, const T* grid, const T* gout, T* gi
         int N, int C, int D, int H, int W, int64_t P, cudaStream_t s) {
   if (N < 0 || C < 0 || D <= 0 || H <= 0 || W <= 0 || P < 0 || !istr) return SR_EINVAL;
   if ((long long)N * P == 0) return SR_OK;
-  if (!input || !grid || !gout || !ginp || !ggrid) return SR_EINVAL;
+  if (!grid || !ggrid || (C > 0 && (!input || !gout || !ginp))) return SR_EINVAL;
   gs3d_bwd_kernel<T><<<sr_grid_for((long long)N * P, kThreads, 16), kThreads, 0, s>>>(
       input, istr[0], istr[1], istr[2], istr[3], istr[4], grid, gout, ginp, ggrid, N, C, D, H, W,
       P);
@@ -246,7 +255,8 @@ int dbwd(const T* ggi, const T* ggg, const T* input, const int64_t* istr, const 
          cudaStream_t s) {
   if (N < 0 || C < 0 || D <= 0 || H <= 0 || W <= 0 || P < 0 || !istr) return SR_EINVAL;
   if ((long long)N * P == 0) return SR_OK;
-  if (!ggi || !ggg || !input || !grid || !gout || !ginp || !ggrid || !ggout) return SR_EINVAL;
+  if (!ggg || !grid || !ggrid || (C > 0 && (!ggi || !input || !gout || !ginp || !ggout)))
+    return SR_EINVAL;
   gs3d_dbwd_kernel<T><<<sr_grid_for((long long)N * P, kThreads, 16), kThreads, 0, s>>>(
       ggi, ggg, input, istr[0], istr[1], istr[2], istr[3], istr[4], grid, gout, ginp, ggrid, ggout,
       N, C, D, H, W, P);

@@ -583,11 +583,28 @@ def _gs_suffix(t):
     raise RuntimeError("grid_sampler_3d: only float32/float64 are supported")
 
 
-def grid_sample3d_forward(inp, grid, want_corner_idx=False):
-    _need_cuda(inp, grid)
+def _gs_shape(inp, grid, *others):
+    """(N, C, D, H, W, P) after the checks the kernels rely on: a 5-D volume, a [N,Do,Ho,Wo,3] grid with the
+    volume's batch size, and every tensor on the volume's device in its dtype (the kernel reads each through a
+    pointer of that type)."""
+    _need_cuda(inp, grid, *others)
+    if inp.dim() != 5 or grid.dim() != 5 or grid.shape[-1] != 3:
+        raise RuntimeError("grid_sampler_3d: expected a volume [N,C,D,H,W] and a grid [N,Do,Ho,Wo,3], got %s and %s"
+                           % (tuple(inp.shape), tuple(grid.shape)))
+    if grid.shape[0] != inp.shape[0]:
+        raise RuntimeError("grid_sampler_3d: volume and grid have batch sizes %d and %d"
+                           % (inp.shape[0], grid.shape[0]))
+    for t in (grid,) + others:
+        if t.dtype != inp.dtype or t.device != inp.device:
+            raise RuntimeError("grid_sampler_3d: expected %s tensors on %s like the volume, got %s on %s"
+                               % (inp.dtype, inp.device, t.dtype, t.device))
     N, Cc, D, H, W = inp.shape
+    return N, Cc, D, H, W, grid.shape[1] * grid.shape[2] * grid.shape[3]
+
+
+def grid_sample3d_forward(inp, grid, want_corner_idx=False):
+    N, Cc, D, H, W, P = _gs_shape(inp, grid)
     Do, Ho, Wo = grid.shape[1:4]
-    P = Do * Ho * Wo
     g = grid.reshape(N, P, 3).contiguous()
     out = torch.empty((N, Cc, Do, Ho, Wo), dtype=inp.dtype, device=inp.device)
     cidx = torch.empty((N, P, 3), dtype=torch.int32, device=inp.device) if want_corner_idx else None
@@ -600,10 +617,7 @@ def grid_sample3d_forward(inp, grid, want_corner_idx=False):
 
 
 def grid_sample3d_backward(inp, grid, grad_output):
-    _need_cuda(inp, grid, grad_output)
-    N, Cc, D, H, W = inp.shape
-    Do, Ho, Wo = grid.shape[1:4]
-    P = Do * Ho * Wo
+    N, Cc, D, H, W, P = _gs_shape(inp, grid, grad_output)
     g = grid.reshape(N, P, 3).contiguous()
     go = grad_output.reshape(N, Cc, P).contiguous()
     ginp = torch.zeros((N, Cc, D, H, W), dtype=inp.dtype, device=inp.device)
@@ -617,10 +631,10 @@ def grid_sample3d_backward(inp, grid, grad_output):
 
 
 def grid_sample3d_dbackward(gg_input, gg_grid, inp, grid, grad_output):
-    _need_cuda(gg_input, gg_grid, inp, grid, grad_output)
-    N, Cc, D, H, W = inp.shape
-    Do, Ho, Wo = grid.shape[1:4]
-    P = Do * Ho * Wo
+    N, Cc, D, H, W, P = _gs_shape(inp, grid, grad_output, gg_input, gg_grid)
+    if gg_input.shape != inp.shape:
+        raise RuntimeError("grid_sampler_3d: gg_input has shape %s, the volume %s"
+                           % (tuple(gg_input.shape), tuple(inp.shape)))
     g = grid.reshape(N, P, 3).contiguous()
     go = grad_output.reshape(N, Cc, P).contiguous()
     ggi = gg_input.contiguous()
