@@ -19,8 +19,10 @@
 //     each, then the epilogue of those rows (bias, activation, forward-mode tangent scaling or
 //     reverse-mode act' multiply, re-split to bf16 planes, tiled store); the epilogue is specialised at
 //     compile time per (activation, rows-per-point, mode);
-//   * 3-stage shared-memory ring (48 KB per stage, 24 KB on the narrow column tile): the bulk copies of the next tile run under the epilogue, the
-//     MMAs do not (both consumer warpgroups are in the epilogue of the same tile; DESIGN.md section 8).
+//   * 3-stage shared-memory ring of 48 KB stages (6 stages of 24 KB on the narrow column tile): the bulk copies of the next tile run under the epilogue, the
+//     MMAs do not (both consumer warpgroups are in the epilogue of the same tile; DESIGN.md section 8).  A reverse
+//     launch also streams the previous layer's activation tiles (act' is recomputed from them) through the ring,
+//     as epilogue stages after each n-tile's k chunks, so the epilogue reads them from shared memory.
 // The FFMA engine (mlp_kernels.cu) stays the accuracy reference; tests compare both.
 #include <cstdlib>
 
@@ -140,19 +142,26 @@ struct EpiRow {
   size_t ds_ld;
 };
 
+// A reverse launch's epilogue reads the previous layer's activation tile of chunk c0 (act' is recomputed from it) only
+// for columns < n; the producer stages exactly these chunks in the operand ring (tc_sweep_kernel), and both sides
+// decide with this one rule.
+__device__ __forceinline__ bool mul_chunk_staged(const LayerArgs& a, int c0) { return c0 < a.n && (c0 >> 5) < a.mul_KC; }
+
 // One 32-column chunk of the accumulator (this thread: one row), layer columns [c0, c0 + 32): bias / activation /
 // tangent scaling (forward) or act' multiply (reverse), then the fp32 outputs, the act' stash and the re-split bf16
 // tile of the next layer.  `live` = the chunk holds GEMM columns (else only the zero padding / skip-connection columns
-// of the next layer's input are produced).
+// of the next layer's input are produced).  `mul_stage` (reverse launches): the ring slot holding this chunk's
+// activation tile (one A stage, both planes), or null when the chunk has no columns < n (act' is then unused).
 template <int ACT, int CH, bool MUL, bool PF = true>
-__device__ __forceinline__ void epi_chunk(const LayerArgs& a, const EpiRow& r, uint32_t (&v)[32], int c0, bool live) {
+__device__ __forceinline__ void epi_chunk(const LayerArgs& a, const EpiRow& r, uint32_t (&v)[32], int c0, bool live,
+                                          const __nv_bfloat16* mul_stage = nullptr) {
   float o[32];
   if (live) {
     if constexpr (MUL) {
       // reverse sweep: delta * act'(z) for the columns that continue; columns >= n (the skip part of
       // a skip layer's input gradient) pass through unscaled.  ACT is the PREVIOUS layer's activation.
-      const __nv_bfloat16* mt = a.mul_tiles + a_tile_off(r.mt, c0 >> 5, a.mul_KC, 0) +
-                                (size_t)(r.row_in_tile >> 3) * 64 + (r.row_in_tile & 7) * 8;
+      const __nv_bfloat16* mt =
+          mul_stage + (size_t)(r.row_in_tile >> 3) * 64 + (r.row_in_tile & 7) * 8;   // shared memory
       const float kk = -144.26950408889634f * a.mul_inv_scale;   // -100 log2(e) / scale
       // optional fp32 act'(z) of the previous layer's VALUE rows (written by its forward launch as `dstash`, row
       // pitch pad256(n)); only chunks with columns < n use act', the skip columns of a skip layer's input have none.
@@ -160,15 +169,20 @@ __device__ __forceinline__ void epi_chunk(const LayerArgs& a, const EpiRow& r, u
       const long long srow = r.row_ok ? (CH == 4 ? (r.row & ~3LL) : r.row) : 0;
       const float* stash = a.dstash == nullptr || c0 >= a.n ? nullptr : a.dstash + (size_t)srow * r.ds_ld + c0;
       const bool use_stash = (ACT == SR_ACT_SOFTPLUS100) && stash != nullptr;
-      // PF: all global operands of the chunk first (8 x 16 B of activation tiles, 8 x 16 B of stash), 16 loads in
-      // flight per thread; PF = false requests them per group of 8 columns (fewer registers)
+      // The activation tile comes from shared memory (staged by the producer's bulk copy under the MMAs).  The fp32
+      // stash of the training sweeps stays a global load, outside the ring: it is row-major with pitch ds_ld, so a
+      // chunk of it is 128 strided 128-byte pieces, not one contiguous bulk copy.  Without a staged tile (no columns
+      // < n) act' is not used: zeros.
+      // PF: all operands of the chunk first (8 x 16 B of activation tiles, 8 x 16 B of stash), 16 loads in flight
+      // per thread; PF = false requests them per group of 8 columns (fewer registers)
+      const uint4 zero4 = make_uint4(0u, 0u, 0u, 0u);
       uint4 q0[PF ? 4 : 1], q1[PF ? 4 : 1];
       float st[PF ? 32 : 1];
       if constexpr (PF) {
 #pragma unroll
         for (int g = 0; g < 4; ++g) {
-          q0[g] = __ldg(reinterpret_cast<const uint4*>(mt + (size_t)g * (BM * 8)));
-          q1[g] = __ldg(reinterpret_cast<const uint4*>(mt + (size_t)g * (BM * 8) + A_PLANE));
+          q0[g] = mul_stage ? *reinterpret_cast<const uint4*>(mt + (size_t)g * (BM * 8)) : zero4;
+          q1[g] = mul_stage ? *reinterpret_cast<const uint4*>(mt + (size_t)g * (BM * 8) + A_PLANE) : zero4;
         }
         if (use_stash) {
 #pragma unroll
@@ -185,8 +199,8 @@ __device__ __forceinline__ void epi_chunk(const LayerArgs& a, const EpiRow& r, u
         if constexpr (PF) {
           a0 = q0[g]; a1 = q1[g];
         } else {
-          a0 = __ldg(reinterpret_cast<const uint4*>(mt + (size_t)g * (BM * 8)));
-          a1 = __ldg(reinterpret_cast<const uint4*>(mt + (size_t)g * (BM * 8) + A_PLANE));
+          a0 = mul_stage ? *reinterpret_cast<const uint4*>(mt + (size_t)g * (BM * 8)) : zero4;
+          a1 = mul_stage ? *reinterpret_cast<const uint4*>(mt + (size_t)g * (BM * 8) + A_PLANE) : zero4;
           if (use_stash) {
             const float4 t0 = __ldg(reinterpret_cast<const float4*>(stash) + 2 * g);
             const float4 t1 = __ldg(reinterpret_cast<const float4*>(stash) + 2 * g + 1);
@@ -335,11 +349,36 @@ constexpr int STG_LD = 132;                 // staging row pitch (floats): confl
 constexpr int STG_FLOATS = 64 * STG_LD;     // per consumer warpgroup: 64 rows x 128 columns
 template <int TBN>
 constexpr uint32_t w_stage_bytes() { return (uint32_t)kPlanes * TBN * BK * 2; }   // 2 planes: 32 KB (TBN 256), 8 KB (64)
+// Ring depth.  The narrow tile's stages are half the size (24 KB) and its MMAs short, so its launches are bound by
+// the A stream; twice the stages keep twice the bytes in flight in the same shared memory as the wide tile's ring.
+template <int TBN>
+constexpr int ring_stages() { return TBN == BN ? STAGES : 2 * STAGES; }
 template <int TBN>
 constexpr size_t smem_bytes() {
-  return (size_t)STAGES * (A_STAGE_BYTES + w_stage_bytes<TBN>()) + (size_t)kConsumerWGs * STG_FLOATS * 4 + 256;
+  return (size_t)ring_stages<TBN>() * (A_STAGE_BYTES + w_stage_bytes<TBN>()) + (size_t)kConsumerWGs * STG_FLOATS * 4 + 256;
 }
-static_assert(smem_bytes<BN>() <= 227 * 1024, "shared memory of one H100 block");
+static_assert(smem_bytes<BN>() <= 227 * 1024 && smem_bytes<BN_NARROW>() <= 227 * 1024, "shared memory of one H100 block");
+static_assert(2 * ring_stages<BN_NARROW>() * sizeof(uint64_t) <= 256, "full + empty barriers fit their 256 bytes");
+
+// Epilogue stages of a reverse launch.  The epilogue runs an n-tile in passes of PASS columns (128, or 64 on the narrow
+// tile); in each pass the warps with (wq >> 1) = q take columns [q PASS / 2, (q + 1) PASS / 2), chunk i = 0 .. WCH - 1
+// in turn, both halves at the same time.  The producer stages the previous layer's activation tile of each chunk
+// (16 KB, both planes: exactly one A stage) in the ring, in that order: on the wide tile one stage carries chunk i of
+// both halves, half 0's in the slot's A part and half 1's in its (32 KB) W part; on the narrow tile (8 KB W part) a
+// stage carries one chunk, half 0's then half 1's.  kEpiHalves = halves per stage.
+template <int TBN>
+constexpr int kEpiHalves = TBN == BN ? 2 : 1;
+static_assert(w_stage_bytes<BN>() >= A_STAGE_BYTES, "the wide tile's W stage holds one activation chunk");
+template <int TBN>
+__device__ __forceinline__ int epi_chunk_col(int nt, int h, int q, int i) {
+  constexpr int PASS = TBN < 128 ? TBN : 128;
+  return nt * TBN + h * PASS + q * (PASS / 2) + 32 * i;
+}
+// where half q's chunk of the stage in ring slot `slot` lands (q0 = the stage's first half)
+template <int TBN>
+__device__ __forceinline__ __nv_bfloat16* epi_stage_dst(__nv_bfloat16* sA, __nv_bfloat16* sW, int slot, int q, int q0) {
+  return q == q0 ? sA + (size_t)slot * A_STAGE : sW + (size_t)slot * (w_stage_bytes<TBN>() / 2);
+}
 
 // One k chunk of this warpgroup's 64 x TBN tile: the split-bf16 product terms, plane pairs smallest contributions
 // first -- 2 planes: (a0,w1) (a1,w0) (a0,w0); 3 planes: (a0,w2) (a2,w0) (a1,w1) (a0,w1) (a1,w0) (a0,w0).
@@ -375,18 +414,19 @@ __device__ __forceinline__ void mma_chunk(float (&acc)[TBN / 2], uint32_t abase,
 template <int ACT, int CH, bool MUL, int TBN>
 __global__ void __launch_bounds__(kThreads, 1) tc_sweep_kernel(const __grid_constant__ LayerArgs a) {
   constexpr uint32_t W_STAGE_BYTES = w_stage_bytes<TBN>();
+  constexpr int NS = ring_stages<TBN>();
   constexpr int W_STAGE = W_STAGE_BYTES / 2;   // elements
   extern __shared__ __align__(1024) unsigned char smem[];
   __nv_bfloat16* sA = reinterpret_cast<__nv_bfloat16*>(smem);
-  __nv_bfloat16* sW = reinterpret_cast<__nv_bfloat16*>(smem + (size_t)STAGES * A_STAGE_BYTES);
-  float* stg = reinterpret_cast<float*>(smem + (size_t)STAGES * (A_STAGE_BYTES + W_STAGE_BYTES));
+  __nv_bfloat16* sW = reinterpret_cast<__nv_bfloat16*>(smem + (size_t)NS * A_STAGE_BYTES);
+  float* stg = reinterpret_cast<float*>(smem + (size_t)NS * (A_STAGE_BYTES + W_STAGE_BYTES));
   uint64_t* bars = reinterpret_cast<uint64_t*>(stg + kConsumerWGs * STG_FLOATS);
-  uint64_t* full = bars;                    // [STAGES] operands of the stage landed (producer expect_tx)
-  uint64_t* empty = bars + STAGES;          // [STAGES] the MMAs of every consumer warp have read the stage
+  uint64_t* full = bars;                    // [NS] operands of the stage landed (producer expect_tx)
+  uint64_t* empty = bars + NS;              // [NS] the MMAs of every consumer warp have read the stage
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7;
   if (threadIdx.x == 0) {
-    for (int i = 0; i < STAGES; ++i) { sr_mbar_init(&full[i], 1); sr_mbar_init(&empty[i], kEpiWarps); }
+    for (int i = 0; i < NS; ++i) { sr_mbar_init(&full[i], 1); sr_mbar_init(&empty[i], kEpiWarps); }
     sr_fence_barrier_init();
   }
   __syncthreads();
@@ -416,7 +456,31 @@ __global__ void __launch_bounds__(kThreads, 1) tc_sweep_kernel(const __grid_cons
             sr_mbar_arrive_expect_tx(&full[slot], A_STAGE_BYTES + W_STAGE_BYTES);
             sr_bulk_g2s(sW + (size_t)slot * W_STAGE, a.W + w_tile_off(TBN, nt, kc, a.KC, 0), W_STAGE_BYTES, &full[slot]);
             sr_bulk_g2s(sA + (size_t)slot * A_STAGE, a.A + a_tile_off(mt, kc, a.KC, 0), A_STAGE_BYTES, &full[slot]);
-            if (++slot == STAGES) { slot = 0; phase ^= 1u; }
+            if (++slot == NS) { slot = 0; phase ^= 1u; }
+          }
+          if constexpr (MUL) {
+            // epilogue stages: the previous layer's activation tiles of the chunks this n-tile's epilogue reads, in
+            // its consumption order (kEpiHalves)
+            constexpr int PASS = TBN < 128 ? TBN : 128, WCH = PASS / 64, EH = kEpiHalves<TBN>;
+            for (int h = 0; h < TBN / PASS; ++h) {
+              for (int i = 0; i < WCH; ++i) {
+                for (int q0 = 0; q0 < 2; q0 += EH) {
+                  uint32_t bytes = 0;
+                  for (int q = q0; q < q0 + EH; ++q)
+                    if (mul_chunk_staged(a, epi_chunk_col<TBN>(nt, h, q, i))) bytes += A_STAGE_BYTES;
+                  if (bytes == 0) continue;
+                  sr_mbar_wait(&empty[slot], phase ^ 1u);
+                  sr_mbar_arrive_expect_tx(&full[slot], bytes);
+                  for (int q = q0; q < q0 + EH; ++q) {
+                    const int c0 = epi_chunk_col<TBN>(nt, h, q, i);
+                    if (mul_chunk_staged(a, c0))
+                      sr_bulk_g2s(epi_stage_dst<TBN>(sA, sW, slot, q, q0),
+                                  a.mul_tiles + a_tile_off(mt, c0 >> 5, a.mul_KC, 0), A_STAGE_BYTES, &full[slot]);
+                  }
+                  if (++slot == NS) { slot = 0; phase ^= 1u; }
+                }
+              }
+            }
           }
         }
       }
@@ -449,7 +513,7 @@ __global__ void __launch_bounds__(kThreads, 1) tc_sweep_kernel(const __grid_cons
                              sr_smem_u32(sW + (size_t)slot * W_STAGE));
         wgmma_commit();
         int prev = slot;
-        if (++slot == STAGES) { slot = 0; phase ^= 1u; }
+        if (++slot == NS) { slot = 0; phase ^= 1u; }
         for (int kc = 1; kc < a.KC; ++kc) {
           sr_mbar_wait(&full[slot], phase);
           wgmma_fence();
@@ -459,7 +523,7 @@ __global__ void __launch_bounds__(kThreads, 1) tc_sweep_kernel(const __grid_cons
           wgmma_wait<1>();   // the previous stage's MMAs are complete: release it
           if (lane == 0) sr_mbar_arrive(&empty[prev]);
           prev = slot;
-          if (++slot == STAGES) { slot = 0; phase ^= 1u; }
+          if (++slot == NS) { slot = 0; phase ^= 1u; }
         }
         wgmma_wait<0>();
         if (lane == 0) sr_mbar_arrive(&empty[prev]);
@@ -478,8 +542,7 @@ __global__ void __launch_bounds__(kThreads, 1) tc_sweep_kernel(const __grid_cons
           }
           warpgroup_sync(1 + cw);
           const float* srow = st + ((wq & 1) * 32 + lane) * STG_LD + (wq >> 1) * (PASS / 2);
-          for (int i = 0; i < WCH; ++i) {
-            const int c0 = nt * TBN + h * PASS + (wq >> 1) * (PASS / 2) + 32 * i;
+          auto chunk = [&](int i, int c0, const __nv_bfloat16* mul_stage) {
             uint32_t v[32];
 #pragma unroll
             for (int j4 = 0; j4 < 8; ++j4) {
@@ -487,7 +550,39 @@ __global__ void __launch_bounds__(kThreads, 1) tc_sweep_kernel(const __grid_cons
               v[4 * j4] = __float_as_uint(t.x); v[4 * j4 + 1] = __float_as_uint(t.y);
               v[4 * j4 + 2] = __float_as_uint(t.z); v[4 * j4 + 3] = __float_as_uint(t.w);
             }
-            epi_chunk<ACT, CH, MUL>(a, r, v, c0, c0 < a.n_gemm);
+            epi_chunk<ACT, CH, MUL>(a, r, v, c0, c0 < a.n_gemm, mul_stage);
+          };
+          if constexpr (!MUL) {
+            for (int i = 0; i < WCH; ++i) chunk(i, nt * TBN + h * PASS + (wq >> 1) * (PASS / 2) + 32 * i, nullptr);
+          } else {
+            // The pass's epilogue stages in ring order (kEpiHalves).  Every warp of both warpgroups waits for every
+            // stage and releases it in that order, reading only its own half's chunk (on the narrow tile a warp
+            // releases the other half's stage unread): the producer refills a slot only after all kEpiWarps warps
+            // released it.  No deadlock: a warp's wait for stage s depends only on releases of stages <= s - NS,
+            // and each warp releases stage s after its wait for s and at most its own chunk's work, never after a
+            // later stage, so the releases of the earliest unreleased stage always complete.  Waiting before a
+            // release also keeps a warp that skips a stage from arriving while the slot's previous use is open.
+            constexpr int EH = kEpiHalves<TBN>;
+            const int qm = wq >> 1;
+            for (int i = 0; i < WCH; ++i) {
+              for (int q0 = 0; q0 < 2; q0 += EH) {
+                bool any = false;
+                for (int q = q0; q < q0 + EH; ++q) any |= mul_chunk_staged(a, epi_chunk_col<TBN>(nt, h, q, i));
+                const bool mine = qm >= q0 && qm < q0 + EH;
+                const int c0 = epi_chunk_col<TBN>(nt, h, qm, i);
+                const __nv_bfloat16* mul_stage = nullptr;
+                if (any) {
+                  sr_mbar_wait(&full[slot], phase);
+                  if (mul_chunk_staged(a, c0)) mul_stage = epi_stage_dst<TBN>(sA, sW, slot, qm, q0);
+                }
+                if (mine) chunk(i, c0, mul_stage);
+                if (any) {
+                  __syncwarp();
+                  if (lane == 0) sr_mbar_arrive(&empty[slot]);
+                  if (++slot == NS) { slot = 0; phase ^= 1u; }
+                }
+              }
+            }
           }
           warpgroup_sync(1 + cw);
         }
