@@ -4,9 +4,12 @@
 //   A = J^T J (symmetric) -> cyclic Jacobi eigen-iteration (fixed 6 sweeps, fp32 storage, the rotation
 //   angles in double so the eigenvalues of a near-identity J keep ~1e-7 relative accuracy)
 //   s_i = sqrt(max(lambda_i, 0)) sorted descending (torch.svd's order), V = matching right singular vectors.
-// Backward of a spectral loss L(s):  dL/dJ = sum_i g_i u_i v_i^T,  u_i = J v_i / s_i  (valid for repeated
-// singular values too: only derivatives of the VALUES are propagated).  Pure HBM stream: 36 B in,
+// Backward of a spectral loss L(s):  dL/dJ = sum_i g_i u_i v_i^T,  u_i = J v_i / s_i, u_2 = det(U) u_0 x u_1 (valid
+// for repeated singular values too: only derivatives of the VALUES are propagated; see svals3x3_bwd_kernel for
+// the terms below FLT_EPSILON * s_max).  Pure HBM stream: 36 B in,
 // 12 (+36) B out per matrix forward; 36 + 12 + 36 + 12 in, 36 out backward.
+#include <cfloat>
+
 #include "common.cuh"
 
 namespace {
@@ -77,14 +80,37 @@ svals3x3_bwd_kernel(const float* __restrict__ J, const float* __restrict__ S, co
     float m[9], v[9], out[9];
 #pragma unroll
     for (int k = 0; k < 9; ++k) { m[k] = J[i * 9 + k]; v[k] = V[i * 9 + k]; out[k] = 0.f; }
+    // u_k = J v_k / s_k carries an absolute error of about FLT_EPSILON * s_max (v_k is stored in fp32), i.e. a relative
+    // error of FLT_EPSILON * s_max / s_k.  So the smallest one is taken as u_2 = det(U) (u_0 x u_1) instead, with
+    // det(U) = sign(det J) det(V) (det J in double from the fp32 entries): accurate however small s_2 is, which keeps
+    // def_regu's restoring term g_2 ~ log(s_2) / s_2 of a collapsing J.  u_0 and u_1 are dropped below FLT_EPSILON * s_max,
+    // where they are noise (and then so is u_2).  The cut is relative: a J of any overall scale keeps its gradient.
+    const float cut = FLT_EPSILON * S[i * 3];
+    float uh[2][3];
 #pragma unroll
     for (int k = 0; k < 3; ++k) {
       const float s = S[i * 3 + k], g = gS[i * 3 + k];
-      const float w = s > 1e-20f ? g / s : 0.f;
       const float vk[3] = {v[k], v[3 + k], v[6 + k]};
       float u[3];
+      if (k < 2) {
+        const float w = s > cut && s > 0.f ? g / s : 0.f;
 #pragma unroll
-      for (int r = 0; r < 3; ++r) u[r] = (m[3 * r] * vk[0] + m[3 * r + 1] * vk[1] + m[3 * r + 2] * vk[2]) * w;
+        for (int r = 0; r < 3; ++r) {
+          const float jv = m[3 * r] * vk[0] + m[3 * r + 1] * vk[1] + m[3 * r + 2] * vk[2];
+          u[r] = jv * w;
+          uh[k][r] = s > cut && s > 0.f ? jv / s : 0.f;
+        }
+      } else {
+        const double detJ = (double)m[0] * ((double)m[4] * m[8] - (double)m[5] * m[7]) -
+                            (double)m[1] * ((double)m[3] * m[8] - (double)m[5] * m[6]) +
+                            (double)m[2] * ((double)m[3] * m[7] - (double)m[4] * m[6]);
+        const float detV = v[0] * (v[4] * v[8] - v[5] * v[7]) - v[1] * (v[3] * v[8] - v[5] * v[6]) +
+                           v[2] * (v[3] * v[7] - v[4] * v[6]);
+        const float sg = ((detJ < 0.0) != (detV < 0.f) ? -1.f : 1.f) * g;
+        u[0] = (uh[0][1] * uh[1][2] - uh[0][2] * uh[1][1]) * sg;
+        u[1] = (uh[0][2] * uh[1][0] - uh[0][0] * uh[1][2]) * sg;
+        u[2] = (uh[0][0] * uh[1][1] - uh[0][1] * uh[1][0]) * sg;
+      }
 #pragma unroll
       for (int r = 0; r < 3; ++r)
 #pragma unroll
