@@ -567,6 +567,15 @@ int sr_tc_trace_update(const int32_t* index, const int32_t* m_dev, int64_t P, fl
 int sr_tc_shade_point(int64_t P, const float* pts, const float* rays, const int64_t* batch_inds,
                       const float* grad, const float* off4, const sr_lbs_params* lbs,
                       float* normals, float* crays, float* dpos, uint8_t* inv_ok, cudaStream_t s);
+/* sr_tc_shade_point_deformed: sr_tc_shade_point's outputs, bit-identical, plus the deformed-surface normal
+ * defnormals [P,3] = normalize(J^-T g) from the same g = grad f (unnormalised) and J = M (I + d offset / dp);
+ * where |det J| < 1e-4 it is normalize(J g), the reference's fallback (utils/utils.py:139-152).  cam_R0 (HOST
+ * [9], row-major, or null) turns it into the debug image's normal diag(-1,1,-1) R0^T n; the reference rotates
+ * every frame of a batch by cameras.R[0] (model/network.py:424), and so does this one. */
+int sr_tc_shade_point_deformed(int64_t P, const float* pts, const float* rays, const int64_t* batch_inds,
+                               const float* grad, const float* off4, const sr_lbs_params* lbs,
+                               float* normals, float* crays, float* dpos, uint8_t* inv_ok, float* defnormals,
+                               const float* cam_R0, cudaStream_t s);
 int sr_tc_render_embed(int64_t P, const float* pts, const float* views, const float* normals,
                        const float* feat, int feat_ld, int feat_col0, int nfeat, int feat_row_stride,
                        int multires, const float* pw, float* out, int ld, cudaStream_t s);

@@ -166,6 +166,8 @@ SIGNATURES = {
     "sr_sdf_forward_indexed": (C.c_int, [C.POINTER(MlpDesc), c_f, i64, c_f, c_f, c_f, stream_t]),
     "sr_tc_shade_point": (C.c_int, [i64, c_f, c_f, c_f, c_f, c_f, C.POINTER(LbsParams), c_f, c_f, c_f, c_f,
                                     stream_t]),
+    "sr_tc_shade_point_deformed": (C.c_int, [i64, c_f, c_f, c_f, c_f, c_f, C.POINTER(LbsParams), c_f, c_f, c_f,
+                                             c_f, c_f, C.POINTER(f32), stream_t]),
     "sr_tc_render_embed": (C.c_int, [i64, c_f, c_f, c_f, c_f, i32, i32, i32, i32, i32, C.POINTER(f32), c_f,
                                      i32, stream_t]),
     "sr_seg3d_candidates": (C.c_int, [c_f, c_f, c_f, i32, i32, i32, i32, i32, i32, i32, i32, i32,

@@ -155,8 +155,14 @@ struct ShadePtArgs {
   float* crays;
   float* dpos;
   unsigned char* inv_ok;
+  float* defn;         // [P][3] deformed normal (DEFORMED instantiation only)
+  float R0[9];         // camera rotation applied to defn when has_R (row-major)
+  int has_R;
 };
 
+// DEFORMED also writes the deformed-surface normal normalize(J^-T g) (fallback normalize(J g) where J is singular,
+// utils/utils.py:139-152) from the grad f and J the cardinal ray already uses; the other outputs are the same code.
+template <bool DEFORMED>
 __global__ void __launch_bounds__(256) shade_point_kernel(const __grid_constant__ ShadePtArgs a) {
   const int lane = threadIdx.x & 31;
   const long long warp0 = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -192,6 +198,28 @@ __global__ void __launch_bounds__(256) shade_point_kernel(const __grid_constant_
       const bool ok = shade_point(a.grad + i * 3, m, a.rays + i * 3, a.normals + i * 3, a.crays + i * 3);
       if (a.dpos) { a.dpos[i * 3] = d[0]; a.dpos[i * 3 + 1] = d[1]; a.dpos[i * 3 + 2] = d[2]; }
       if (a.inv_ok) a.inv_ok[i] = ok ? 1 : 0;
+      if constexpr (DEFORMED) {
+        const float g[3] = {a.grad[i * 3], a.grad[i * 3 + 1], a.grad[i * 3 + 2]};
+        float c[9], det, n[3];
+        if (minv3x3_cofactors(m, c, det)) {
+          // (J^-1)^T g with J^-1[r][k] = c[3k+r] / det, as shade_point applies J^-1 to v
+#pragma unroll
+          for (int r = 0; r < 3; ++r) n[r] = (c[3 * r] / det) * g[0] + (c[3 * r + 1] / det) * g[1] + (c[3 * r + 2] / det) * g[2];
+        } else {
+#pragma unroll
+          for (int r = 0; r < 3; ++r) n[r] = m[3 * r] * g[0] + m[3 * r + 1] * g[1] + m[3 * r + 2] * g[2];
+        }
+        const float nn = sqrtf(n[0] * n[0] + n[1] * n[1] + n[2] * n[2]);
+        n[0] /= nn; n[1] /= nn; n[2] /= nn;
+        if (a.has_R) {
+          // diag(-1, 1, -1) R0^T n: the image's normal (model/network.py:424)
+          float t[3];
+#pragma unroll
+          for (int r = 0; r < 3; ++r) t[r] = a.R0[r] * n[0] + a.R0[3 + r] * n[1] + a.R0[6 + r] * n[2];
+          n[0] = -t[0]; n[1] = t[1]; n[2] = -t[2];
+        }
+        a.defn[i * 3] = n[0]; a.defn[i * 3 + 1] = n[1]; a.defn[i * 3 + 2] = n[2];
+      }
     }
   }
 }
@@ -247,7 +275,24 @@ int sr_tc_shade_point(int64_t P, const float* pts, const float* rays, const int6
   a.off4 = off4; a.has_lbs = lbs ? 1 : 0;
   if (lbs) a.lbs = *lbs;
   a.normals = normals; a.crays = crays; a.dpos = dpos; a.inv_ok = inv_ok;
-  shade_point_kernel<<<sr_grid_for(P * 32, 256, 8), 256, 0, s>>>(a);
+  a.defn = nullptr; a.has_R = 0;
+  shade_point_kernel<false><<<sr_grid_for(P * 32, 256, 8), 256, 0, s>>>(a);
+  return sr_launch_status();
+}
+
+int sr_tc_shade_point_deformed(int64_t P, const float* pts, const float* rays, const int64_t* batch_inds,
+                               const float* grad, const float* off4, const sr_lbs_params* lbs,
+                               float* normals, float* crays, float* dpos, uint8_t* inv_ok, float* defnormals,
+                               const float* cam_R0, cudaStream_t s) {
+  if (P <= 0 || !pts || !rays || !grad || !normals || !crays || !defnormals) return SR_EINVAL;
+  ShadePtArgs a;
+  a.P = P; a.pts = pts; a.rays = rays; a.batch_inds = (const long long*)batch_inds; a.grad = grad;
+  a.off4 = off4; a.has_lbs = lbs ? 1 : 0;
+  if (lbs) a.lbs = *lbs;
+  a.normals = normals; a.crays = crays; a.dpos = dpos; a.inv_ok = inv_ok;
+  a.defn = defnormals; a.has_R = cam_R0 ? 1 : 0;
+  for (int q = 0; q < 9; ++q) a.R0[q] = cam_R0 ? cam_R0[q] : 0.f;
+  shade_point_kernel<true><<<sr_grid_for(P * 32, 256, 8), 256, 0, s>>>(a);
   return sr_launch_status();
 }
 

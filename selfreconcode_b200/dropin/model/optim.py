@@ -12,6 +12,7 @@ caller or from an injected `raster_seed` callable and then run exactly the refer
 No-grad evaluations run on the fused kernels; losses that need a graph use the modules' autograd
 path (same math as torch ops on the GPU).
 """
+import os
 import os.path as osp
 
 import numpy as np
@@ -476,12 +477,18 @@ class OptimNetwork(nn.Module):
             self.TmpVid, self.TmpFid = vertex_face_pairs(self.Tmpfs, self.TmpVs.shape[0])
             self.mesh_reg_topo = None
             self.root = root
+        oldTmpVs = self.TmpVs.detach().clone() if self.root else None
         poses, trans, d_cond, _ = self.dataset.get_grad_parameters(frame_ids, device)
         defconds = [d_cond, [poses, trans]]
         defTmpVs = self._deform(self.TmpVs[None, :, :].expand(N, -1, 3), defconds, None, ratio)
+        # the translator offset of this deform, for the snapshot's def1 meshes (later calls overwrite defs[0].offset)
+        offset = self.deformer.defs[0].offset.detach().view(N, -1, 3) if self.root else None
         with torch.no_grad():
             bi, ri, ci, ps, _ = self._mesh_seed(defTmpVs, self.TmpVs, self.Tmpfs)
-        pc_loss = self._pc_silhouette_loss(defTmpVs, defconds, gtMs, H, W, ratio)
+        pc_loss, masks, mgtMs = self._pc_silhouette_loss(defTmpVs, defconds, gtMs, H, W, ratio)
+        if self.root:
+            self.save_debug(oldTmpVs, self.Tmpfs, defTmpVs, offset, masks, gtMs, mgtMs, datas, bi, ri, ci, ps,
+                            [d_cond.detach(), [poses.detach(), trans.detach()]], ratio, cameras)
         sel = gtMs[bi, ri, ci] > 0.      # colour losses only where render mask and gt mask intersect
         bi, ri, ci, ps = bi[sel], ri[sel], ci[sel], ps[sel]
         sample_pix = self.conf.get_int('sample_pix_num') if 'sample_pix_num' in self.conf else sample_pix
@@ -503,12 +510,13 @@ class OptimNetwork(nn.Module):
     def _pc_silhouette_loss(self, defTmpVs, defconds, gtMs, H, W, ratio):
         """network.py:497-507: soft point-cloud silhouette of the deformed template vs the (dilated) gt
         mask, then computeTmpPcLoss.  Without a point renderer (no level applied yet, none injected) the term is
-        unavailable: that is an error unless `allow_missing_pc_loss` is set -- never a silent omission."""
+        unavailable: that is an error unless `allow_missing_pc_loss` is set -- never a silent omission.
+        -> (loss, point-cloud masks, dilated gt mask or None when the radius rounds to 0)."""
         self.info['pc_loss'] = {}
         if self.pcRender is None:
             if getattr(self, "allow_missing_pc_loss", False):
                 self.info['pc_loss']['skipped'] = True
-                return torch.zeros((), device=defTmpVs.device)
+                return torch.zeros((), device=defTmpVs.device), None, None
             raise RuntimeError("OptimNetwork.forward: no point renderer (pcRender) -- install pytorch3d, inject one, "
                                "or set allow_missing_pc_loss=True to train without the silhouette term")
         N, V = defTmpVs.shape[0], self.TmpVs.shape[0]
@@ -524,10 +532,89 @@ class OptimNetwork(nn.Module):
             masks, _ = self.pcRender(P.Pointclouds(points=meshes.verts_list(), features=feats))
             radius = self.pcRender.rasterizer.raster_settings.radius
         radius = int(np.round(radius / 2. * float(min(H, W)) / 1.2))
-        target = gtMs
+        mgtMs = None
         if radius > 0:
-            target = torch.nn.functional.max_pool2d(gtMs, kernel_size=2 * radius + 1, stride=1, padding=radius)
-        return self.computeTmpPcLoss(meshes, defconds, masks, target, ratio)
+            mgtMs = torch.nn.functional.max_pool2d(gtMs, kernel_size=2 * radius + 1, stride=1, padding=radius)
+        loss = self.computeTmpPcLoss(meshes, defconds, masks, gtMs if mgtMs is None else mgtMs, ratio)
+        return loss, masks, mgtMs
+
+    # ---- network.py:374-447 ---------------------------------------------------------------------
+    def save_debug(self, TmpVs, Tmpfs, defTmpVs, offset, masks, gtMs, mgtMs, datas, batch_inds, row_inds, col_inds,
+                   initTmpPs, defconds, ratio, cameras):
+        """The progress snapshot of a remesh step, written under self.root: tmp.ply (the template before the inner
+        SGD step), def_i.ply (deformed template of frame i), def1_i.ply (template + translator offset), m_i.png (point
+        silhouette), mgm_i.png (dilated gt mask, when the radius is above 0) and, when self.draw is set, rgb_i.png /
+        gtrgb_i.png / normal_i.png: the traced colour and the deformed-surface normal of every covered pixel.
+        Builds no graph that outlives it, writes no .grad and draws no random numbers, so the step's loss and gradients do
+        not depend on it."""
+        if self.root is None:
+            return
+        import cv2
+        from . import snapshot as S
+        root = self.root
+        os.makedirs(root, exist_ok=True)
+        with torch.no_grad():
+            S.write_ply(osp.join(root, 'tmp.ply'), TmpVs, Tmpfs)
+            for ind in range(defTmpVs.shape[0]):
+                S.write_ply(osp.join(root, 'def_%d.ply' % ind), defTmpVs[ind], Tmpfs)
+            for ind in range(offset.shape[0]):
+                S.write_ply(osp.join(root, 'def1_%d.ply' % ind), TmpVs + offset[ind], Tmpfs)
+            if masks is not None:
+                for ind, img in enumerate(S.mask_image(masks)):
+                    cv2.imwrite(osp.join(root, 'm%d.png' % ind), img)
+            if mgtMs is not None:
+                for ind, img in enumerate(S.mask_image(mgtMs)):
+                    cv2.imwrite(osp.join(root, 'mgm%d.png' % ind), img)
+            if not self.draw:
+                return
+            gtCs = datas['img'].to(initTmpPs.device)
+            print('draw %d points' % initTmpPs.shape[0])
+            tcolors, tnormals = self._draw_rays(batch_inds, row_inds, col_inds, initTmpPs, cameras, defconds, ratio)
+            colors = S.color_image(tcolors, batch_inds, row_inds, col_inds, gtCs)
+            normals = S.normal_image(tnormals, batch_inds, row_inds, col_inds, gtCs)
+            gtcolors = S.gt_color_image(gtCs)
+            for ind in range(colors.shape[0]):
+                cv2.imwrite(osp.join(root, 'rgb%d.png' % ind), colors[ind])
+                cv2.imwrite(osp.join(root, 'gtrgb%d.png' % ind), gtcolors[ind])
+                cv2.imwrite(osp.join(root, 'normal%d.png' % ind), normals[ind])
+        self.draw = False
+
+    def _draw_rays(self, batch_inds, row_inds, col_inds, initTmpPs, cameras, defconds, ratio, chunk=1 << 18):
+        """Colour and camera-frame deformed normal of every seed pixel (network.py:405-424): trace as infer_rays does,
+        then one shading pass per chunk that also returns the deformed normal.  The reference turns the normals of
+        every frame by cameras.R[0]; so does this.  -> ([P,3] colours, [P,3] normals)"""
+        pix = torch.cat([col_inds.view(-1, 1), row_inds.view(-1, 1), torch.ones_like(col_inds.view(-1, 1))], dim=-1)
+        rays = cameras.view_rays(pix.float())
+        cam_pos = cameras.cam_pos().detach()
+        R0 = cameras.R[0].detach()
+        tcolors, tnormals = [], []
+        for rays_, ps_, bi_ in zip(torch.split(rays, chunk), torch.split(initTmpPs, chunk), torch.split(batch_inds, chunk)):
+            with torch.enable_grad():
+                # user-supplied field modules trace by autograd w.r.t. the points (FindSurfacePs._optimize_generic); the
+                # fused tracer builds no graph either way.  Neither writes .grad.
+                ps_, _ = utils.OptimizeSurfacePs(cam_pos, rays_.detach(), ps_.clone(), bi_, self.sdf, ratio,
+                                                 self.deformer, defconds, dthreshold=1.e-4, athreshold=self.angThred,
+                                                 w1=3.05, w2=1., times=30)
+            ps_ = ps_.detach()
+            if hasattr(self.sdf, "forward_fused"):
+                _, _, rgb, nx = utils.shade_rays(self.sdf, self.deformer, self.netRender, ps_, rays_, defconds, bi_,
+                                                 ratio, deformed_normals=True, cam_R0=R0)
+            else:
+                # user-supplied field modules: infer_rays' autograd sequence for the colour, then the deformed normal
+                with torch.enable_grad():
+                    ps_ = ps_.requires_grad_(True)
+                    sdfs = self.sdf(ps_, ratio)
+                    n0 = torch.autograd.grad(sdfs, ps_, torch.ones_like(sdfs))[0]
+                    n0 = n0 / n0.norm(dim=1, keepdim=True)
+                    crays, defVs = utils.compute_cardinal_rays(self.deformer, ps_, rays_, defconds, bi_, ratio, 'test')
+                    nx, _ = utils.compute_deformed_normals(self.sdf, self.deformer, ps_, defconds, bi_, ratio, 'test')
+                self.sdf(ps_, ratio)          # rendcond of these points, without a graph
+                rgb = utils.compute_netRender_color(self.netRender, ps_, defVs, n0, crays, self.sdf.rendcond, None,
+                                                    ratio)
+                nx = utils.camera_normals(nx.detach(), R0)
+            tcolors.append(rgb)
+            tnormals.append(nx)
+        return torch.cat(tcolors, dim=0), torch.cat(tnormals, dim=0)
 
     # ---- network.py:647-697 ---------------------------------------------------------------------
     def computeTmpPcLoss(self, defMeshes, defconds, imgs, gtMs, ratio):

@@ -191,12 +191,21 @@ def compute_netRender_color(net, ps, ds, ns, vs, features, framefeatures, ratio)
     return net(ps, ns, vs, features, ratio)
 
 
-def shade_rays(sdf, deformer, netRender, ps, rays, defconds, batch_inds, ratio):
+def camera_normals(nx, R0):
+    """The debug image's normal diag(-1,1,-1) R0^T n of every row of nx [P,3] (model/network.py:424)."""
+    flip = torch.tensor([[-1., 0., 0.], [0., 1., 0.], [0., 0., -1.]], device=nx.device)
+    return (flip @ R0.transpose(0, 1) @ nx.view(-1, 3, 1)).view(-1, 3)
+
+
+def shade_rays(sdf, deformer, netRender, ps, rays, defconds, batch_inds, ratio, deformed_normals=False, cam_R0=None):
     """Everything the infer loop does with a traced point (model/network.py:356-368): template
     normal grad f / |grad f|, cardinal ray J^-1 v, rendered colour.  -> (normals, crays, rgb), no
     graph.  Large batches with the stock field modules run the SDF / translator sweeps (value +
     3 forward tangents), the pointwise geometry and the rendering network back to back on the
-    tensor-core engine (ops.shade_and_render_tc); otherwise the per-op fused kernels are used."""
+    tensor-core engine (ops.shade_and_render_tc); otherwise the per-op fused kernels are used.
+    With `deformed_normals` a fourth output is the deformed-surface normal normalize(J^-T grad f) (the debug
+    snapshot's, model/network.py:420-424), turned by camera_normals when a 3x3 `cam_R0` is given: on the
+    tensor-core path it comes out of the same pointwise pass; otherwise from compute_deformed_normals(..., 'test')."""
     P = ps.shape[0]
     stock = (_fusable(deformer) and hasattr(sdf, "fused") and hasattr(netRender, "fused")
              and getattr(netRender, "mode", None) == 'idr' and getattr(netRender, "multires_n", 1) == 0
@@ -210,14 +219,19 @@ def shade_rays(sdf, deformer, netRender, ps, rays, defconds, batch_inds, ratio):
             lbs = sk.lbs_state()
             lbs.set_pose(poses.view(poses.shape[0], 24, 3), trans)
             nfeat = full.desc.layer[full.desc.n_layers - 1].n - 1
-            n, cr, rgb, _, _ = ops.shade_and_render_tc(full, tr.fused(ratio), lbs, netRender.fused(ratio), ps, rays,
-                                                       batch_inds, defconds[0], nfeat=nfeat)
-            return n, cr, rgb
+            out = ops.shade_and_render_tc(full, tr.fused(ratio), lbs, netRender.fused(ratio), ps, rays, batch_inds,
+                                          defconds[0], nfeat=nfeat, deformed_normals=deformed_normals, cam_R0=cam_R0)
+            return (out[0], out[1], out[2], out[5]) if deformed_normals else out[:3]
         _, nx, feat = sdf.forward_fused(ps, ratio, want_grad=True, want_feat=True)
         nx = nx / nx.norm(dim=1, keepdim=True)
         crays, defVs = compute_cardinal_rays(deformer, ps, rays, defconds, batch_inds, ratio, 'test')
         rgb = compute_netRender_color(netRender, ps, defVs, nx, crays, feat, None, ratio)
-    return nx, crays, rgb
+        if not deformed_normals:
+            return nx, crays, rgb
+        dn, _ = compute_deformed_normals(sdf, deformer, ps, defconds, batch_inds, ratio, 'test')
+        if cam_R0 is not None:
+            dn = camera_normals(dn, cam_R0)
+    return nx, crays, rgb, dn
 
 
 # ------------------------------------------------------------------------------------------------

@@ -1533,11 +1533,14 @@ def _sdf_grad_tc(lib, sdf_full, pts, P):
     return out, grad, g_out
 
 
-def shade_and_render_tc(sdf_full, def_net, lbs, render_net, pts, rays, batch_inds, conds, nfeat=256):
+def shade_and_render_tc(sdf_full, def_net, lbs, render_net, pts, rays, batch_inds, conds, nfeat=256,
+                        deformed_normals=False, cam_R0=None):
     """Shading of the infer path on the tensor-core engine: grad f of the SDF in reverse mode (one value-only forward
     sweep + one reverse sweep), the translator's sweep with forward tangents (4 rows per point: its 3x3 Jacobian),
     pointwise geometry, then the rendering network.
-    Returns (normals, cardinal rays, rgb, D(p), inverse-ok mask)."""
+    Returns (normals, cardinal rays, rgb, D(p), inverse-ok mask); with `deformed_normals` also the deformed-surface
+    normal normalize(J^-T grad f) [P,3] from the same pointwise pass, rotated into the debug image's frame
+    diag(-1,1,-1) cam_R0^T n when a 3x3 `cam_R0` is given."""
     _need_cuda(pts, rays)
     dev = pts.device
     P = pts.shape[0]
@@ -1563,8 +1566,17 @@ def shade_and_render_tc(sdf_full, def_net, lbs, render_net, pts, rays, batch_ind
         crays = torch.empty((P, 3), dtype=torch.float32, device=dev)
         dpos = torch.empty((P, 3), dtype=torch.float32, device=dev)
         ok = torch.empty((P,), dtype=torch.bool, device=dev)
-        check(lib.sr_tc_shade_point(P, _p(pts), _p(rays), _p(bi), _p(grad), _p(o4), _lbs_ref(lbs),
-                                    _p(normals), _p(crays), _p(dpos), _p(ok), _stream()), "tc_shade_point")
+        if deformed_normals:
+            defn = torch.empty((P, 3), dtype=torch.float32, device=dev)
+            R0 = None
+            if cam_R0 is not None:
+                R0 = (C.c_float * 9)(*[float(x) for x in cam_R0.detach().reshape(9).float().cpu().tolist()])
+            check(lib.sr_tc_shade_point_deformed(P, _p(pts), _p(rays), _p(bi), _p(grad), _p(o4), _lbs_ref(lbs),
+                                                 _p(normals), _p(crays), _p(dpos), _p(ok), _p(defn), R0, _stream()),
+                  "tc_shade_point_deformed")
+        else:
+            check(lib.sr_tc_shade_point(P, _p(pts), _p(rays), _p(bi), _p(grad), _p(o4), _lbs_ref(lbs),
+                                        _p(normals), _p(crays), _p(dpos), _p(ok), _stream()), "tc_shade_point")
         rd = render_net.desc
         ld = _pad(rd.d_in, 32)
         emb = torch.empty((P, ld), dtype=torch.float32, device=dev)
@@ -1574,4 +1586,6 @@ def shade_and_render_tc(sdf_full, def_net, lbs, render_net, pts, rays, batch_ind
         rn = tc_net(render_net)
         rgb = torch.empty((P, rn.layers[-1]["n"]), dtype=torch.float32, device=dev)
         _tc_mlp(lib, rn, emb, 1, rgb)
+    if deformed_normals:
+        return normals, crays, rgb, dpos, ok, defn
     return normals, crays, rgb, dpos, ok
