@@ -16,7 +16,7 @@ import torch.nn.functional as F
 
 from selfreconcode_b200 import ops
 from .Embedder import get_embedder
-from ._fused import FoldCache, needs_autograd, ratio_value, require_cuda, SR_ACT_NONE, SR_ACT_RELU
+from ._fused import FoldCache, index_rows, needs_autograd, ratio_value, require_cuda, SR_ACT_NONE, SR_ACT_RELU
 
 
 def _mm(a, b):
@@ -76,7 +76,7 @@ class CompositeDeformer(nn.Module):
             n, v = ps.shape[0], ps.shape[1]
             cond_rows = conds[0].view(n, 1, -1).expand(n, v, conds[0].shape[-1]).reshape(n * v, -1)
         else:
-            cond_rows = conds[0].index_select(0, batch_inds)
+            cond_rows = index_rows(conds[0], batch_inds)
         pts = ps.reshape(-1, 3)
         off, Joff = tr.forward_train(pts, cond_rows, ratio, want_jac)
         tr.offset = off.view(shape)
@@ -192,7 +192,7 @@ class MLPTranslator(nn.Module):
                 ws = [w for w in ops.annealing_weights(self.multires, ratio) for _ in (0, 1)]
                 ps = self.embed_fn(ps, ws)
         if batch_inds is not None:
-            x = torch.cat([ps, conds.index_select(0, batch_inds)], dim=1)
+            x = torch.cat([ps, index_rows(conds, batch_inds)], dim=1)
         else:
             c = conds.view(-1, 1, self.feature_vector_size).expand(-1, ps.shape[1], -1)
             x = torch.cat([ps, c], dim=-1).view(-1, ps.shape[-1] + self.feature_vector_size)
@@ -332,9 +332,9 @@ class LBSkinner(nn.Module):
         # one gather instead of the reference's per-frame masked loop with a host sync per frame
         # (Deformer.py:226-231): T_p = sum_j w_pj A[b_p, j]
         # (broadcast multiply + sum instead of einsum / matmul: no cuBLAS launches in the training step)
-        T = (ps_ws.unsqueeze(-1) * A.view(batch_size, 24, 16).index_select(0, batch_inds)).sum(1).view(-1, 4, 4)
+        T = (ps_ws.unsqueeze(-1) * index_rows(A.view(batch_size, 24, 16), batch_inds)).sum(1).view(-1, 4, 4)
         v = (T[:, :3, :] * F.pad(ps, (0, 1), mode='constant', value=1).unsqueeze(-2)).sum(-1)
-        return v + trans.index_select(0, batch_inds)
+        return v + index_rows(trans, batch_inds)
 
 
 def smooth_weights(weights, times=3):

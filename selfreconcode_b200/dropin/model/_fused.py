@@ -15,6 +15,33 @@ def needs_autograd(*tensors):
     return torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in tensors)
 
 
+class _IndexRows(torch.autograd.Function):
+    """t.index_select(0, idx) whose backward sums the rows of each index in a fixed order (index_put with accumulate,
+    sorted by index on CUDA) instead of index_select's atomicAdd: a step's per-frame gradients (poses, translations,
+    latent codes) are then bit-identical from run to run.  The backward is itself differentiable."""
+
+    @staticmethod
+    def forward(ctx, t, idx):
+        ctx.save_for_backward(idx)
+        ctx.n = t.shape[0]
+        return t.index_select(0, idx)
+
+    @staticmethod
+    def backward(ctx, g):
+        idx, = ctx.saved_tensors
+        return scatter_rows(g, idx, ctx.n), None
+
+
+def index_rows(t, idx):
+    """Rows idx of t (dim 0), deterministic in the backward."""
+    return _IndexRows.apply(t, idx)
+
+
+def scatter_rows(src, idx, n):
+    """[n, ...] with out[i] = sum of the rows src[j] with idx[j] == i, summed in a fixed order (differentiable)."""
+    return src.new_zeros((n,) + tuple(src.shape[1:])).index_put((idx,), src, accumulate=True)
+
+
 def require_cuda(t, what):
     if not t.is_cuda:
         raise RuntimeError("%s: CUDA tensor required -- selfrecon_b200 has no CPU path" % what)

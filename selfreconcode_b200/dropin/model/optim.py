@@ -24,6 +24,7 @@ from FastMinv import Fast3x3Minv
 import MCGpu
 from selfreconcode_b200 import ops
 from .CameraMine import RectifiedPerspectiveCameras, PointsRendererWithFrags
+from ._fused import scatter_rows
 
 
 def _p3d():
@@ -51,10 +52,10 @@ def vertex_face_pairs(faces, n_verts):
 
 
 def _scatter_mean(src, index, n):
-    """torch_scatter.scatter(..., reduce='mean', dim_size=n) (network.py:617,637)."""
-    s = torch.zeros((n,) + tuple(src.shape[1:]), dtype=src.dtype, device=src.device).index_add(0, index, src)
-    c = torch.zeros(n, dtype=src.dtype, device=src.device).index_add(
-        0, index, torch.ones_like(index, dtype=src.dtype)).clamp(min=1)
+    """torch_scatter.scatter(..., reduce='mean', dim_size=n) (network.py:617,637), summed in a fixed order so that the
+    step's loss is bit-identical from run to run."""
+    s = scatter_rows(src, index, n)
+    c = scatter_rows(torch.ones_like(index, dtype=src.dtype), index, n).clamp(min=1)
     return s / c.view((-1,) + (1,) * (src.dim() - 1))
 
 

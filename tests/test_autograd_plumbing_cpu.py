@@ -105,3 +105,21 @@ def test_upsample_wrapper_gradient(monkeypatch):
     out, flag = Interp2xBoundary3d(0.1)(x)
     assert out.shape == (1, 1, 5, 7, 5) and flag.dtype == torch.bool and not flag.requires_grad
     assert torch.autograd.gradcheck(lambda t: Interp2xBoundary3dFunction.apply(t, 0.1)[0], (x,), eps=1e-6, atol=1e-6)
+
+
+def test_index_rows_first_and_second_order():
+    """model/_fused.index_rows (the per-point gather of per-frame poses, translations and latent codes) and
+    scatter_rows (the per-frame mean of the ray losses): the values of index_select / a per-frame sum, and first- and
+    second-order gradcheck in float64."""
+    H.dropin()
+    from model._fused import index_rows, scatter_rows
+    g = torch.Generator().manual_seed(0)
+    t = torch.randn(3, 4, 5, dtype=torch.float64, generator=g).requires_grad_(True)
+    idx = torch.tensor([2, 0, 2, 2, 1, 0, 2])
+    assert torch.equal(index_rows(t, idx), t.index_select(0, idx))
+    assert torch.autograd.gradcheck(lambda t: index_rows(t, idx), (t,))
+    assert torch.autograd.gradgradcheck(lambda t: index_rows(t, idx) ** 2, (t,))
+    s = torch.randn(7, 2, dtype=torch.float64, generator=g).requires_grad_(True)
+    ref = torch.stack([s[idx == i].sum(0) for i in range(4)])
+    assert torch.allclose(scatter_rows(s, idx, 4), ref, rtol=0, atol=1e-15)
+    assert torch.autograd.gradcheck(lambda s: scatter_rows(s, idx, 4) ** 2, (s,))
