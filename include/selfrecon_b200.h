@@ -514,23 +514,6 @@ int sr_svals3x3_f32(const float* J, float* S, float* V, int64_t n, cudaStream_t 
 int sr_svals3x3_bwd_f32(const float* J, const float* S, const float* V, const float* gS, float* gJ, int64_t n,
                         cudaStream_t s);
 
-/* Weight-normalised layers (torch.nn.utils.weight_norm, dim 0; model/network.py:60-61, model/RenderNet.py): the
- * effective weights w = g v / ||v|| of up to 12 layers in one launch, and the backward of that map
- * (gv, gg from gw; gw may be NULL = no gradient reached this layer, gw_ld = row stride of gw in floats).
- * inv_norm [n] is written by the forward call and read by the backward call. */
-typedef struct sr_wn_layer {
-  const float* v;       /* [n][k] direction parameter (weight_v) */
-  const float* g;       /* [n] magnitude parameter (weight_g) */
-  float* w;             /* [n][k] effective weight (forward out) */
-  float* inv_norm;      /* [n] 1 / ||v|| (forward out, backward in) */
-  const float* gw;      /* [n][gw_ld] gradient of w (backward in) or NULL */
-  float* gv;            /* [n][k] (backward out) */
-  float* gg;            /* [n] (backward out) */
-  int32_t n, k, gw_ld, pad_;
-} sr_wn_layer;
-int sr_weight_norm_forward(const sr_wn_layer* layers, int L, cudaStream_t s);
-int sr_weight_norm_backward(const sr_wn_layer* layers, int L, cudaStream_t s);
-
 /* Borderline decisions.  The tensor-core engine's values carry up to ~2.4e-5 of absolute error, so
  * a sign (`> balance`, MCAcc/seg3d_lossless.py:333-346) or threshold (`< dthreshold`,
  * utils/FindSurfacePs.py:120-127) decision on a value inside that band is re-taken on the fp32 FFMA engine:

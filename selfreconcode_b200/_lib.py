@@ -45,13 +45,6 @@ class TcLayer(C.Structure):
                 ("n", C.c_int), ("k", C.c_int), ("act", C.c_int), ("skip", C.c_int)]
 
 
-class WnLayer(C.Structure):
-    """struct sr_wn_layer (weight-norm forward / backward over several layers)."""
-    _fields_ = [("v", C.c_void_p), ("g", C.c_void_p), ("w", C.c_void_p), ("inv_norm", C.c_void_p),
-                ("gw", C.c_void_p), ("gv", C.c_void_p), ("gg", C.c_void_p),
-                ("n", C.c_int32), ("k", C.c_int32), ("gw_ld", C.c_int32), ("pad_", C.c_int32)]
-
-
 class TraceParams(C.Structure):
     _fields_ = [("cam_pos", C.c_float * 3), ("dthreshold", C.c_float), ("athreshold", C.c_float),
                 ("w1", C.c_float), ("w2", C.c_float)]
@@ -156,8 +149,6 @@ SIGNATURES = {
     "sr_tc_wgrad": (C.c_int, [c_f, i32, c_f, i32, i64, c_f, c_f, i32, i32, i32, stream_t]),
     "sr_tc_colsum": (C.c_int, [c_f, i64, i32, i32, c_f, i32, stream_t]),
     "sr_tc_unpack_rows": (C.c_int, [c_f, i64, i32, i32, c_f, i32, stream_t]),
-    "sr_weight_norm_forward": (C.c_int, [C.POINTER(WnLayer), i32, stream_t]),
-    "sr_weight_norm_backward": (C.c_int, [C.POINTER(WnLayer), i32, stream_t]),
     "sr_svals3x3_f32": (C.c_int, [c_f, c_f, c_f, i64, stream_t]),
     "sr_svals3x3_bwd_f32": (C.c_int, [c_f, c_f, c_f, c_f, c_f, i64, stream_t]),
     "sr_band_select": (C.c_int, [c_f, i64, f32, f32, c_f, c_f, stream_t]),

@@ -13,9 +13,8 @@ CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIBNAME = "libselfrecon_b200.so"
 SOURCES = ["minv3x3.cu", "marching_cubes.cu", "interp2x.cu", "grid_sampler.cu", "mlp_kernels.cu",
-           "seg3d.cu", "tc_gemm.cu", "trace_tc.cu", "svals3x3.cu", "tc_wgrad.cu", "raster.cu", "weight_norm.cu",
-           "mesh_shade.cu", "points_silhouette.cu", "texture_bake.cu", "lbsw_field.cu",
-           "mesh_reg.cu", "frames.cu"]
+           "seg3d.cu", "tc_gemm.cu", "trace_tc.cu", "svals3x3.cu", "tc_wgrad.cu", "raster.cu", "mesh_shade.cu",
+           "points_silhouette.cu", "texture_bake.cu", "lbsw_field.cu", "mesh_reg.cu", "frames.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 

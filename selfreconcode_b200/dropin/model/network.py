@@ -9,6 +9,8 @@ forward().  Execution:
     torch ops on the GPU.  (Fused backward kernels are the next step; see DESIGN.md.)
 CPU tensors are rejected: there is no CPU path.
 """
+import contextlib
+
 import numpy as np
 import torch
 import torch.nn as nn
@@ -56,6 +58,7 @@ class ImplicitNetwork(nn.Module):
         self.softplus = nn.Softplus(beta=100)
         self.rendcond = None
         self._cache = FoldCache()
+        self._weff = None     # the layers' effective weights inside shared_weights()
 
     # ---- fused engine --------------------------------------------------------------------
     def _layers(self):
@@ -112,41 +115,35 @@ class ImplicitNetwork(nn.Module):
             # large value-only batches (the 257^3 / 513^3 grid queries): tensor-core engine
             # (wgmma split-BF16 GEMM per layer, csrc/tc_gemm.cu)
             sdf = ops.tc_mlp_forward(net, pts, ch=1, n_out=1)
-            if refine_about is not None and ops.TC_REFINE:
+            if refine_about is not None:
                 ops.sdf_refine_band(net, pts.contiguous().float(), sdf.view(-1), float(refine_about))
             return sdf.view(-1, 1), None, None
         sdf, grad, feat = ops.sdf_forward(net, pts, want_grad, nfeat)
         return sdf.view(-1, 1), grad, feat
 
     # ---- fused training path (tensor-core engine, forward tangents) --------------------------
+    @contextlib.contextmanager
     def shared_weights(self):
-        """Context manager: evaluations inside it share ONE set of effective (weight-normed) weight tensors, i.e. one
+        """Evaluations inside this context share ONE set of effective (weight-normed) weight tensors, i.e. one
         weight-norm sub-graph for several forward_train calls that are back-propagated together."""
-        net = self
+        self._weff = self._weights()
+        try:
+            yield
+        finally:
+            self._weff = None
 
-        class _Ctx:
-            def __enter__(self):
-                net._weff = {}
-
-            def __exit__(self, *a):
-                net._weff = None
-
-        return _Ctx()
+    def _weights(self):
+        """The effective weight of every layer, in layer order."""
+        from selfreconcode_b200 import train_ops as T
+        lins = [getattr(self, "lin" + str(l)) for l in range(self.num_layers - 1)]
+        return T.weight_norm_all(lins) if self.weight_norm else [lin.weight for lin in lins]
 
     def _effective(self, l):
         from selfreconcode_b200 import train_ops as T
+        if self._weff is not None:
+            return self._weff[l]
         lin = getattr(self, "lin" + str(l))
-        if not self.weight_norm:
-            return lin.weight
-        cache = getattr(self, "_weff", None)
-        if cache is None:
-            return T.weight_norm_eff(lin.weight_v, lin.weight_g)
-        if l not in cache:
-            # all layers in one launch (and one backward launch) the first time any of them is asked for
-            L = self.num_layers - 1
-            for i, W in enumerate(T.weight_norm_all([getattr(self, "lin" + str(i)) for i in range(L)])):
-                cache[i] = W
-        return cache[l]
+        return T.weight_norm_eff(lin.weight_v, lin.weight_g) if self.weight_norm else lin.weight
 
     def _train_ok(self):
         from selfreconcode_b200 import train_ops
@@ -165,14 +162,7 @@ class ImplicitNetwork(nn.Module):
         ch = 4 if want_grad else 1
         L = self.num_layers - 1
         Ws, bs, acts, skips = [], [], [], []
-        local = self.weight_norm and getattr(self, "_weff", None) is None
-        if local:
-            self._weff = {}          # this call's own weight-norm sub-graph (one fused launch)
-        try:
-            Weff = [self._effective(l) for l in range(L)]
-        finally:
-            if local:
-                self._weff = None
+        Weff = self._weff if self._weff is not None else self._weights()
         for l in range(L):
             lin = getattr(self, "lin" + str(l))
             W = Weff[l]

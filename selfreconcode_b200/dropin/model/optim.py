@@ -12,6 +12,7 @@ caller or from an injected `raster_seed` callable and then run exactly the refer
 No-grad evaluations run on the fused kernels; losses that need a graph use the modules' autograd
 path (same math as torch ops on the GPU).
 """
+import contextlib
 import os
 import os.path as osp
 
@@ -279,8 +280,6 @@ class OptimNetwork(nn.Module):
         stands for the template vertices the reference adds to the eikonal sample set (:543)."""
         device = frame_ids.device
         conf = self.conf
-        if getattr(self.sdf, "_weff", None) is not None:
-            self.sdf._weff = None        # a previous call that raised must not leave its weight sub-graph behind
         gtCs = datas['img'].to(device)
         N = gtCs.shape[0]
         cameras, H, W = self._cameras(N, device)
@@ -301,83 +300,81 @@ class OptimNetwork(nn.Module):
         nonmnfld_pnts.requires_grad_()
         fused_train = utils.train_fused(self.deformer, self.sdf) and self.netRender._train_ok() \
             if hasattr(self.netRender, "_train_ok") else False
-        import contextlib
         shared = self.sdf.shared_weights() if fused_train else contextlib.nullcontext()
-        shared.__enter__()       # eikonal and surface-point evaluations share one weight-norm sub-graph
-        if fused_train:
-            # eikonal term on the tensor-core training engine: grad f is a forward-mode output (network.py:545-547)
-            _, grad, _ = self.sdf.forward_train(nonmnfld_pnts, ratio, want_grad=True, want_feat=False)
-        else:
-            pred = self.sdf(nonmnfld_pnts, ratio)
-            grad = self.sdf.gradient(nonmnfld_pnts, pred)
-        grad_loss = ((grad.norm(2, dim=-1) - 1) ** 2).mean()
-        self.info['grad_loss'] = grad_loss.item()
-        total_loss = total_loss + grad_loss * conf.get_float('grad_weight')
-        total_loss = total_loss + self._regularisers(nonmnfld_pnts, base, N, d_cond, poses, trans, ratio, frame_ids)
-        self.info['color_loss'] = -1.0
-        self._tmp_geom = None
-        if self.info['rayInfo'][1] > 0:
-            self.TmpPs = initTmpPs[check]
-            self.TmpPs.requires_grad = True
-            self.rays = rays[check]
-            self.batch_inds = batch_inds[check]
-            self.col_inds = col_inds[check]
-            self.row_inds = row_inds[check]
-            grad_d_p = None
+        with shared:       # eikonal and surface-point evaluations share one weight-norm sub-graph
             if fused_train:
-                # f, grad f, rendcond in one forward-mode sweep; D(p), dD/dp in another (network.py:606-610)
-                sdfs, gf_raw, rendcond_p = self.sdf.forward_train(self.TmpPs, ratio, want_grad=True, want_feat=True)
-                self.sdf.rendcond = rendcond_p
-                nx = gf_raw / gf_raw.norm(dim=1, keepdim=True)
-                defVs, grad_d_p = self.deformer.forward_train(self.TmpPs, defconds, self.batch_inds, ratio, True)
-                # grad f and dD/dp at the surface points, reused (detached) by the normal weights below and by
-                # propagateTmpPsGrad: the reference re-evaluates both there (network.py:625, 721-748)
-                self._tmp_geom = (self.TmpPs, gf_raw.detach(), grad_d_p.detach())
-                Jinv, inv_mask = utils.FastDiff3x3MinvFunction.apply(grad_d_p)
-                crays = utils.mv3(Jinv, self.rays.view(-1, 3))
-                crays = torch.where(inv_mask.view(-1, 1), crays, self.rays.detach())
-                crays = crays / crays.norm(dim=1, keepdim=True)
+                # eikonal term on the tensor-core training engine: grad f is a forward-mode output (network.py:545-547)
+                _, grad, _ = self.sdf.forward_train(nonmnfld_pnts, ratio, want_grad=True, want_feat=False)
             else:
-                sdfs = self.sdf(self.TmpPs, ratio)
-                nx = torch.autograd.grad(sdfs, self.TmpPs, torch.ones_like(sdfs), retain_graph=True,
-                                         create_graph=True)[0]
-                nx = nx / nx.norm(dim=1, keepdim=True)
-                crays, defVs = utils.compute_cardinal_rays(self.deformer, self.TmpPs, self.rays, defconds,
-                                                           self.batch_inds, ratio, 'train')
-            if conf.get_float('color_weight') > 0.:
-                colors = utils.compute_netRender_color(self.netRender, self.TmpPs, defVs, nx, crays, self.sdf.rendcond,
-                                                       None, ratio)
-                color_loss = (gtCs[self.batch_inds, self.row_inds, self.col_inds, :] - colors).abs().sum(1)
-                color_loss = _scatter_mean(color_loss, self.batch_inds, N).mean()
-                self.info['color_loss'] = color_loss.item()
-                total_loss = total_loss + conf.get_float('color_weight') * color_loss
-            if 'normal' in datas and 'normal_weight' in conf and conf.get_float('normal_weight') > 0.:
-                if 'weighted_normal' in conf and conf.get_bool('weighted_normal'):
-                    if self._tmp_geom is not None:
-                        cnx = utils.deformed_normals_from(self._tmp_geom[1], self._tmp_geom[2])
+                pred = self.sdf(nonmnfld_pnts, ratio)
+                grad = self.sdf.gradient(nonmnfld_pnts, pred)
+            grad_loss = ((grad.norm(2, dim=-1) - 1) ** 2).mean()
+            self.info['grad_loss'] = grad_loss.item()
+            total_loss = total_loss + grad_loss * conf.get_float('grad_weight')
+            total_loss = total_loss + self._regularisers(nonmnfld_pnts, base, N, d_cond, poses, trans, ratio, frame_ids)
+            self.info['color_loss'] = -1.0
+            self._tmp_geom = None
+            if self.info['rayInfo'][1] > 0:
+                self.TmpPs = initTmpPs[check]
+                self.TmpPs.requires_grad = True
+                self.rays = rays[check]
+                self.batch_inds = batch_inds[check]
+                self.col_inds = col_inds[check]
+                self.row_inds = row_inds[check]
+                grad_d_p = None
+                if fused_train:
+                    # f, grad f, rendcond in one forward-mode sweep; D(p), dD/dp in another (network.py:606-610)
+                    sdfs, gf_raw, rendcond_p = self.sdf.forward_train(self.TmpPs, ratio, want_grad=True, want_feat=True)
+                    self.sdf.rendcond = rendcond_p
+                    nx = gf_raw / gf_raw.norm(dim=1, keepdim=True)
+                    defVs, grad_d_p = self.deformer.forward_train(self.TmpPs, defconds, self.batch_inds, ratio, True)
+                    # grad f and dD/dp at the surface points, reused (detached) by the normal weights below and by
+                    # propagateTmpPsGrad: the reference re-evaluates both there (network.py:625, 721-748)
+                    self._tmp_geom = (self.TmpPs, gf_raw.detach(), grad_d_p.detach())
+                    Jinv, inv_mask = utils.FastDiff3x3MinvFunction.apply(grad_d_p)
+                    crays = utils.mv3(Jinv, self.rays.view(-1, 3))
+                    crays = torch.where(inv_mask.view(-1, 1), crays, self.rays.detach())
+                    crays = crays / crays.norm(dim=1, keepdim=True)
+                else:
+                    sdfs = self.sdf(self.TmpPs, ratio)
+                    nx = torch.autograd.grad(sdfs, self.TmpPs, torch.ones_like(sdfs), retain_graph=True,
+                                             create_graph=True)[0]
+                    nx = nx / nx.norm(dim=1, keepdim=True)
+                    crays, defVs = utils.compute_cardinal_rays(self.deformer, self.TmpPs, self.rays, defconds,
+                                                               self.batch_inds, ratio, 'train')
+                if conf.get_float('color_weight') > 0.:
+                    colors = utils.compute_netRender_color(self.netRender, self.TmpPs, defVs, nx, crays,
+                                                           self.sdf.rendcond, None, ratio)
+                    color_loss = (gtCs[self.batch_inds, self.row_inds, self.col_inds, :] - colors).abs().sum(1)
+                    color_loss = _scatter_mean(color_loss, self.batch_inds, N).mean()
+                    self.info['color_loss'] = color_loss.item()
+                    total_loss = total_loss + conf.get_float('color_weight') * color_loss
+                if 'normal' in datas and 'normal_weight' in conf and conf.get_float('normal_weight') > 0.:
+                    if 'weighted_normal' in conf and conf.get_bool('weighted_normal'):
+                        if self._tmp_geom is not None:
+                            cnx = utils.deformed_normals_from(self._tmp_geom[1], self._tmp_geom[2])
+                        else:
+                            cnx, _ = utils.compute_deformed_normals(self.sdf, self.deformer, self.TmpPs, defconds,
+                                                                    self.batch_inds, ratio, 'test')
+                        weights = torch.clamp((-self.rays * cnx.detach()).sum(1).detach(), max=1., min=0.) ** 2
                     else:
-                        cnx, _ = utils.compute_deformed_normals(self.sdf, self.deformer, self.TmpPs, defconds,
-                                                                self.batch_inds, ratio, 'test')
-                    weights = torch.clamp((-self.rays * cnx.detach()).sum(1).detach(), max=1., min=0.) ** 2
-                else:
-                    weights = torch.ones(nx.shape[0], device=device)
-                gtn = datas['normal'].to(device)[self.batch_inds, self.row_inds, self.col_inds, :]
-                flip = torch.tensor([[-1., 0., 0.], [0., 1., 0.], [0., 0., -1.]], device=device)
-                gtn = utils.mv3((cameras.R[0] * flip.diagonal().view(1, 3)).unsqueeze(0), gtn.view(-1, 3))
-                gtnorms = gtn.norm(dim=1, keepdim=True)
-                valid = (gtnorms > 0.0001)[..., 0]
-                gtn = torch.where(valid.view(-1, 1), gtn / gtnorms.clamp(min=1e-12), gtn)
-                if grad_d_p is not None:
-                    J = grad_d_p               # the forward-mode Jacobian of the sweep above
-                else:
-                    ds = self.deformer(self.TmpPs, defconds, self.batch_inds, ratio=ratio)
-                    J = utils.compute_Jacobian(self.TmpPs, ds, True, True)
-                gtn = utils.mtv3(J, gtn.view(-1, 3))
-                normal_loss = (gtn - nx).norm(2, dim=1) * weights
-                normal_loss = _scatter_mean(normal_loss[valid], self.batch_inds[valid], N).mean()
-                self.info['normal_loss'] = normal_loss.item()
-                total_loss = total_loss + conf.get_float('normal_weight') * normal_loss
-        shared.__exit__(None, None, None)
+                        weights = torch.ones(nx.shape[0], device=device)
+                    gtn = datas['normal'].to(device)[self.batch_inds, self.row_inds, self.col_inds, :]
+                    flip = torch.tensor([[-1., 0., 0.], [0., 1., 0.], [0., 0., -1.]], device=device)
+                    gtn = utils.mv3((cameras.R[0] * flip.diagonal().view(1, 3)).unsqueeze(0), gtn.view(-1, 3))
+                    gtnorms = gtn.norm(dim=1, keepdim=True)
+                    valid = (gtnorms > 0.0001)[..., 0]
+                    gtn = torch.where(valid.view(-1, 1), gtn / gtnorms.clamp(min=1e-12), gtn)
+                    if grad_d_p is not None:
+                        J = grad_d_p               # the forward-mode Jacobian of the sweep above
+                    else:
+                        ds = self.deformer(self.TmpPs, defconds, self.batch_inds, ratio=ratio)
+                        J = utils.compute_Jacobian(self.TmpPs, ds, True, True)
+                    gtn = utils.mtv3(J, gtn.view(-1, 3))
+                    normal_loss = (gtn - nx).norm(2, dim=1) * weights
+                    normal_loss = _scatter_mean(normal_loss[valid], self.batch_inds[valid], N).mean()
+                    self.info['normal_loss'] = normal_loss.item()
+                    total_loss = total_loss + conf.get_float('normal_weight') * normal_loss
         if count_step:
             self.forward_time += 1
         return total_loss

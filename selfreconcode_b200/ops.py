@@ -23,12 +23,10 @@ TC_ENABLED = _os.environ.get("SELFRECON_B200_TC", "1") != "0"
 # 2048: below it a tensor-core trace is launch bound and the fp32 engine (one persistent kernel) is the faster choice
 TC_MIN_POINTS = int(_os.environ.get("SELFRECON_B200_TC_MIN_POINTS", "2048"))
 
-# The tensor-core engine's error bounds (DESIGN.md section 4): TC_EPS_F bounds its absolute error on an SDF value
+# The tensor-core engine's error bound (DESIGN.md section 4): TC_EPS_F bounds its absolute error on an SDF value
 # (split-BF16 with fp32 accumulation, csrc/tc_gemm.cu), and sign decisions inside it are re-taken on the fp32 FFMA
-# engine (sdf_refine_band); TC_EPS_A (degrees) is the error of the ray/point angle that follows from D(p)'s.
-TC_EPS_F = float(_os.environ.get("SELFRECON_B200_TC_EPS_F", "4e-5"))
-TC_EPS_A = float(_os.environ.get("SELFRECON_B200_TC_EPS_A", "1e-3"))
-TC_REFINE = _os.environ.get("SELFRECON_B200_TC_REFINE", "1") != "0"
+# engine (sdf_refine_band).
+TC_EPS_F = 4e-5
 TC_DUAL_STREAM = _os.environ.get("SELFRECON_B200_TC_DUAL_STREAM", "1") != "0"
 
 import itertools as _it
@@ -799,7 +797,6 @@ def sdf_forward(net, pts, want_grad=False, nfeat=0):
 
 
 _band_scratch = {}
-SMALL_REFINE = _os.environ.get("SELFRECON_B200_SMALL_REFINE", "1") != "0"
 SMALL_CAP = 4096
 _KERNELS_PER_CALL["sdf_forward_small"] = 10
 
@@ -823,27 +820,23 @@ def sdf_refine_band(net, pts, sdf, center=0.0, eps=None):
         cnt, lst = buf[0:1], buf[1:]
         cnt.zero_()
         check(lib.sr_band_select(_p(sdf), P, float(center), eps, _p(lst), _p(cnt), _stream()), "band_select")
-        if SMALL_REFINE:
-            # short lists: one column-split launch per layer instead of the persistent engine's per-tile latency;
-            # the list is longer than SMALL_CAP only in degenerate cases -- then the persistent engine takes all of it
-            wkey = key + ("small",)
-            work = _band_scratch.get(wkey)
-            if work is None:
-                work = torch.empty((lib.sr_sdf_small_work_bytes(SMALL_CAP),), dtype=torch.uint8, device=dev)
-                _band_scratch[wkey] = work
-            check(lib.sr_sdf_forward_small(C.byref(net.desc), _p(pts), P, _p(lst), _p(cnt), _p(sdf), _p(work),
-                                           SMALL_CAP, _stream()), "sdf_forward_small")
-            over = _band_scratch.get(key + ("over",))
-            if over is None:
-                over = torch.empty((1,), dtype=torch.int32, device=dev)
-                _band_scratch[key + ("over",)] = over
-            torch.clamp(cnt - SMALL_CAP, min=0, out=over)
-            if P > SMALL_CAP:
-                check(lib.sr_sdf_forward_indexed(C.byref(net.desc), _p(pts), P, _p(lst[SMALL_CAP:]), _p(over), _p(sdf),
-                                                 _stream()), "sdf_forward_indexed")
-        else:
-            check(lib.sr_sdf_forward_indexed(C.byref(net.desc), _p(pts), P, _p(lst), _p(cnt), _p(sdf), _stream()),
-                  "sdf_forward_indexed")
+        # short lists: one column-split launch per layer instead of the persistent engine's per-tile latency;
+        # the list is longer than SMALL_CAP only in degenerate cases -- then the persistent engine takes the rest
+        wkey = key + ("small",)
+        work = _band_scratch.get(wkey)
+        if work is None:
+            work = torch.empty((lib.sr_sdf_small_work_bytes(SMALL_CAP),), dtype=torch.uint8, device=dev)
+            _band_scratch[wkey] = work
+        check(lib.sr_sdf_forward_small(C.byref(net.desc), _p(pts), P, _p(lst), _p(cnt), _p(sdf), _p(work),
+                                       SMALL_CAP, _stream()), "sdf_forward_small")
+        over = _band_scratch.get(key + ("over",))
+        if over is None:
+            over = torch.empty((1,), dtype=torch.int32, device=dev)
+            _band_scratch[key + ("over",)] = over
+        torch.clamp(cnt - SMALL_CAP, min=0, out=over)
+        if P > SMALL_CAP:
+            check(lib.sr_sdf_forward_indexed(C.byref(net.desc), _p(pts), P, _p(lst[SMALL_CAP:]), _p(over), _p(sdf),
+                                             _stream()), "sdf_forward_indexed")
     return sdf
 
 

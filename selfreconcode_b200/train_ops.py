@@ -311,84 +311,11 @@ def weight_norm_eff(v, g):
     return v * (g.view(-1, 1) / v.norm(dim=1, keepdim=True))
 
 
-class WeightNormAllFunction(torch.autograd.Function):
-    """Effective weights of several weight-normalised layers: ONE launch forward (sr_weight_norm_forward), ONE launch
-    backward (sr_weight_norm_backward) instead of ~12 element-wise / reduce launches per layer per direction.
-    Inputs v0, g0, v1, g1, ... (weight_v [n,k], weight_g [n,1]); outputs W0, W1, ... (views of one buffer)."""
-
-    @staticmethod
-    def forward(ctx, *vg):
-        lib = _lib.load()
-        L = len(vg) // 2
-        vs = [vg[2 * i].detach().contiguous().float() for i in range(L)]
-        gs = [vg[2 * i + 1].detach().reshape(-1).contiguous().float() for i in range(L)]
-        dev = vs[0].device
-        nk = [tuple(v.shape) for v in vs]
-        wbuf = torch.empty((sum(n * k for n, k in nk),), dtype=torch.float32, device=dev)
-        inv = torch.empty((sum(n for n, _ in nk),), dtype=torch.float32, device=dev)
-        arr = (_lib.WnLayer * L)()
-        outs, o, r = [], 0, 0
-        for i, (n, k) in enumerate(nk):
-            w = wbuf[o:o + n * k].view(n, k)
-            c = arr[i]
-            c.v, c.g, c.w, c.inv_norm = vs[i].data_ptr(), gs[i].data_ptr(), w.data_ptr(), inv[r:r + n].data_ptr()
-            c.gw, c.gv, c.gg, c.n, c.k, c.gw_ld = None, None, None, n, k, k
-            outs.append(w)
-            o += n * k
-            r += n
-        with torch.cuda.device(dev):
-            check(lib.sr_weight_norm_forward(arr, L, torch.cuda.current_stream().cuda_stream), "weight_norm_forward")
-        ctx.save_for_backward(inv, *vs, *gs)
-        ctx.nk = nk
-        ctx.g_shapes = [vg[2 * i + 1].shape for i in range(L)]
-        return tuple(outs)
-
-    @staticmethod
-    @torch.autograd.function.once_differentiable
-    def backward(ctx, *gws):
-        lib = _lib.load()
-        saved = ctx.saved_tensors
-        inv = saved[0]
-        L = len(ctx.nk)
-        vs, gs = saved[1:1 + L], saved[1 + L:1 + 2 * L]
-        dev = inv.device
-        gvbuf = torch.empty((sum(n * k for n, k in ctx.nk),), dtype=torch.float32, device=dev)
-        ggbuf = torch.empty((sum(n for n, _ in ctx.nk),), dtype=torch.float32, device=dev)
-        arr = (_lib.WnLayer * L)()
-        keep, res, o, r = [], [], 0, 0
-        for i, (n, k) in enumerate(ctx.nk):
-            gw = gws[i]
-            if gw is not None and (gw.dtype != torch.float32 or gw.stride(1) != 1):
-                gw = gw.float().contiguous()
-            keep.append(gw)
-            gv, gg = gvbuf[o:o + n * k].view(n, k), ggbuf[r:r + n]
-            c = arr[i]
-            c.v, c.g, c.w, c.inv_norm = vs[i].data_ptr(), gs[i].data_ptr(), None, inv[r:r + n].data_ptr()
-            c.gw = gw.data_ptr() if gw is not None else None
-            c.gv, c.gg, c.n, c.k, c.gw_ld = gv.data_ptr(), gg.data_ptr(), n, k, (gw.stride(0) if gw is not None else k)
-            res += [gv, gg.view(ctx.g_shapes[i])]
-            o += n * k
-            r += n
-        with torch.cuda.device(dev):
-            check(lib.sr_weight_norm_backward(arr, L, torch.cuda.current_stream().cuda_stream), "weight_norm_backward")
-        return tuple(res)
-
-
 import os as _os
 
-# Off by default: parity-tested (tests/test_gpu_train.py) and 360 launches fewer per optimisation step, but the one
-# bench run with it on showed a slower optimizer phase that was never bisected (DESIGN.md section 8).
-FUSED_WEIGHT_NORM = _os.environ.get("SELFRECON_B200_FUSED_WN", "0") != "0"
 
-
-def weight_norm_all(lins, fused=None):
-    """Effective weights of a list of weight-normalised torch Linear modules (weight_v / weight_g), in layer order.
-    CUDA parameters: one fused launch per direction for up to 12 layers; otherwise the element-wise torch form."""
-    if lins and (FUSED_WEIGHT_NORM if fused is None else fused) and lins[0].weight_v.is_cuda and len(lins) <= 12:
-        vg = []
-        for lin in lins:
-            vg += [lin.weight_v, lin.weight_g]
-        return list(WeightNormAllFunction.apply(*vg))
+def weight_norm_all(lins):
+    """Effective weights of a list of weight-normalised torch Linear modules (weight_v / weight_g), in layer order."""
     return [weight_norm_eff(lin.weight_v, lin.weight_g) for lin in lins]
 
 

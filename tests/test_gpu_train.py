@@ -179,41 +179,3 @@ def test_embed_kernels_match_torch_embedding(cuda_dev):
         assert norm_err(outs[True][1].cpu().numpy(), outs[False][1].cpu().numpy()) < 1e-5
         if E:
             assert norm_err(outs[True][2].cpu().numpy(), outs[False][2].cpu().numpy()) < 1e-6
-
-
-def test_fused_weight_norm_matches_torch(cuda_dev):
-    """sr_weight_norm_forward / backward (all layers of a network in one launch) against the element-wise torch form
-    of torch.nn.utils.weight_norm (model/network.py:60-61): effective weights and the gradients of v and g, with one
-    layer whose weights get no gradient and one whose gradient arrives as a row slice (the value-only SDF head)."""
-    from selfreconcode_b200 import train_ops as T
-    g = torch.Generator().manual_seed(11)
-    shapes = [(512, 39), (512, 512), (473, 512), (257, 512), (3, 256)]
-    lins = []
-    for n, k in shapes:
-        lin = torch.nn.Linear(k, n)
-        lin.weight.data = torch.randn(n, k, generator=g) * 0.05
-        lins.append(torch.nn.utils.weight_norm(lin).to(cuda_dev))
-    coef = [torch.randn(n, k, generator=g).to(cuda_dev) for n, k in shapes]
-
-    def loss_of(Ws):
-        tot = (Ws[0] * coef[0]).sum() + (Ws[1] * coef[1]).pow(2).sum() + (Ws[2] * coef[2]).sum()
-        tot = tot + (Ws[3][:1] * coef[3][:1]).sum()          # row slice: the rest of the layer gets zeros
-        return tot                                            # Ws[4] unused: no gradient reaches it
-
-    res = {}
-    for fused in (True, False):
-        for lin in lins:
-            lin.weight_v.grad = None
-            lin.weight_g.grad = None
-        Ws = T.weight_norm_all(lins, fused=True) if fused else [T.weight_norm_eff(l.weight_v, l.weight_g) for l in lins]
-        loss_of(Ws).backward()
-        res[fused] = ([w.detach().clone() for w in Ws],
-                      [(l.weight_v.grad, l.weight_g.grad) for l in lins])
-    for a, b in zip(res[True][0], res[False][0]):
-        assert torch.allclose(a, b, rtol=2e-6, atol=1e-9)
-    for i, ((gv, gg), (hv, hg)) in enumerate(zip(res[True][1], res[False][1])):
-        if hv is None:
-            assert gv is None or float(gv.abs().max()) == 0.0
-            continue
-        assert (gv - hv).abs().max().item() <= 2e-5 * hv.abs().max().item() + 1e-9, i
-        assert (gg - hg).abs().max().item() <= 2e-5 * hg.abs().max().item() + 1e-9, i
