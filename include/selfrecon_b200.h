@@ -587,6 +587,33 @@ int sr_seg3d_scatter(const int64_t* lin, int64_t n, const float* values, const f
                      float balance, float* grid, uint8_t* conflict, int64_t conflict_bytes,
                      int32_t* n_conflicts, cudaStream_t s);
 
+/* ------------------------------------------------------------------------------------------
+ * Front-normal network of the normal-map step (generate_normals.py:116-166; csrc/normal_net.cu).  Activations are
+ * fp32 channels-last [B,H,W,C]; a convolution is sr_conv_pack + sr_tc_linear over row chunks.
+ *   sr_conv_pack: rows [row0, row0+rows) of the implicit im2col matrix of a kh x kw convolution, column
+ *       k = (ky*kw + kx)*Cin + ci, row m = (b*Ho + oy)*Wo + ox, into the tiled split-bf16 layout of
+ *       sr_tc_pack_rows (sr_tc_act_bytes(rows, kh*kw*Cin) bytes; tile rows past `rows` are zero).  Zero or
+ *       reflection (reflect = 1, pad < H, W) padding, stride 1 or 2; transposed = 1 is ConvTranspose2d in gather
+ *       form: input (oy + pad - ky) / stride when that divides exactly and lies in range, else zero.
+ *   sr_instance_norm_stats: mean and 1/sqrt(biased var + 1e-5) [B][C] of y [B][HW][C]; float64 partial sums over
+ *       fixed 512-pixel slices (scratch: sr_instance_norm_partial_bytes), added in a fixed order: deterministic, and
+ *       a sample's result does not depend on B.
+ *   sr_instance_norm_apply: out = relu?((y - mean) * rstd) (+ residual), all [B][HW][C]; out may alias y or residual.
+ *   sr_normal_unwarp: net output [B,S,S,3] sampled back onto B frames of H x W through the crop boxes [B,4]
+ *       (x, y, w, h as floats) as grid_sample(bilinear, zeros, align_corners=True) with x' = 2(c - x)/w - 1, then
+ *       generate_normals.py:155-165: |n| < 1e-4 or background -> 0, else (n*0.5 + 0.5)[::-1]*255 truncated:
+ *       uint8 BGR [B,H,W,3].  fg (uint8 [B,H,W], nonzero = foreground) may be NULL (no mask).
+ * ------------------------------------------------------------------------------------------ */
+int sr_conv_pack(const float* x, int B, int H, int W, int Cin, int kh, int kw, int stride, int pad, int reflect,
+                 int transposed, int Ho, int Wo, int64_t row0, int64_t rows, void* dst, cudaStream_t s);
+int64_t sr_instance_norm_partial_bytes(int B, int64_t HW, int C);
+int sr_instance_norm_stats(const float* y, int B, int64_t HW, int C, void* partial, float* mean, float* rstd,
+                           cudaStream_t s);
+int sr_instance_norm_apply(const float* y, int B, int64_t HW, int C, const float* mean, const float* rstd,
+                           const float* residual, int relu, float* out, cudaStream_t s);
+int sr_normal_unwarp(const float* net, int B, int S, const float* boxes, const uint8_t* fg, int H, int W,
+                     uint8_t* out, cudaStream_t s);
+
 #ifdef __cplusplus
 }
 #endif

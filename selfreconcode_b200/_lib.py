@@ -166,6 +166,12 @@ SIGNATURES = {
     "sr_seg3d_gather": (C.c_int, [c_f, i64, i32, i32, i32, i32, i32, i32, i32, i32, C.POINTER(f32), C.POINTER(f32),
                                   c_f, c_f, c_f, c_f, stream_t]),
     "sr_seg3d_scatter": (C.c_int, [c_f, i64, c_f, c_f, f32, c_f, c_f, i64, c_f, stream_t]),
+    "sr_conv_pack": (C.c_int, [c_f, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, i64, i64, c_f,
+                               stream_t]),
+    "sr_instance_norm_partial_bytes": (i64, [i32, i64, i32]),
+    "sr_instance_norm_stats": (C.c_int, [c_f, i32, i64, i32, c_f, c_f, c_f, stream_t]),
+    "sr_instance_norm_apply": (C.c_int, [c_f, i32, i64, i32, c_f, c_f, c_f, i32, c_f, stream_t]),
+    "sr_normal_unwarp": (C.c_int, [c_f, i32, i32, c_f, c_f, i32, i32, c_f, stream_t]),
 }
 
 _lib = None

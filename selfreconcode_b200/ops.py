@@ -1582,3 +1582,117 @@ def shade_and_render_tc(sdf_full, def_net, lbs, render_net, pts, rays, batch_ind
     if deformed_normals:
         return normals, crays, rgb, dpos, ok, defn
     return normals, crays, rgb, dpos, ok
+
+
+# ------------------------------------------------------------------------------------------------
+# Front-normal network (csrc/normal_net.cu; generate_normals.py:116-166): convolutions as an implicit-im2col pack
+# plus the tensor-core layer kernel, instance norm, and the map of the net output back onto the frame
+# ------------------------------------------------------------------------------------------------
+class TcConv:
+    """One convolution on the tensor-core engine: weight [Cout, Cin, kh, kw] (Conv2d) or [Cin, Cout, kh, kw]
+    (ConvTranspose2d, transposed=True) reordered once to [Cout, kh*kw*Cin] (tap-major, channel-minor) and packed;
+    bias zero-padded to pad256(Cout).  pad_mode 'zeros' or 'reflect'; output_padding only for transposed."""
+
+    def __init__(self, weight, bias, stride=1, pad=0, pad_mode="zeros", transposed=False, output_padding=0):
+        _need_cuda(weight)
+        w = weight.detach().float()
+        if transposed:
+            w = w.permute(1, 2, 3, 0)           # W[ci, co, ky, kx] -> [co, ky, kx, ci]
+        else:
+            w = w.permute(0, 2, 3, 1)           # W[co, ci, ky, kx] -> [co, ky, kx, ci]
+        self.cout, self.kh, self.kw, self.cin = (int(s) for s in w.shape)
+        self.K = self.kh * self.kw * self.cin
+        self.W = tc_pack_weights(w.reshape(self.cout, self.K))
+        self.bias = torch.zeros((_pad(self.cout, 256),), dtype=torch.float32, device=w.device)
+        if bias is not None:
+            self.bias[:self.cout] = bias.detach().float().reshape(-1)
+        if pad_mode not in ("zeros", "reflect") or stride not in (1, 2):
+            raise ValueError("TcConv: stride 1 or 2, pad_mode 'zeros' or 'reflect'")
+        self.stride, self.pad, self.reflect = int(stride), int(pad), pad_mode == "reflect"
+        self.transposed, self.output_padding = bool(transposed), int(output_padding)
+
+    def out_size(self, H, W):
+        if self.transposed:
+            f = lambda n, k: (n - 1) * self.stride - 2 * self.pad + k + self.output_padding
+        else:
+            f = lambda n, k: (n + 2 * self.pad - k) // self.stride + 1
+        return f(H, self.kh), f(W, self.kw)
+
+    def row_bytes(self):
+        return _lib.load().sr_tc_act_bytes(128, self.K) // 128
+
+
+def conv2d(x, conv, workspace, act=_lib.SR_ACT_NONE, chunk_rows=None, out=None):
+    """x fp32 channels-last [B,H,W,Cin] -> conv(x) fp32 [B,Ho,Wo,Cout] (act applied), through row chunks of the
+    implicit im2col matrix packed into `workspace` (a uint8 CUDA buffer): each chunk is one sr_conv_pack and one
+    sr_tc_linear.  chunk_rows (a multiple of 128) defaults to what the workspace holds."""
+    _need_cuda(x, workspace)
+    B, H, W, Cin = (int(s) for s in x.shape)
+    if Cin != conv.cin or x.dtype != torch.float32 or not x.is_contiguous():
+        raise ValueError("conv2d: expected contiguous fp32 [B,H,W,%d], got %s %s" % (conv.cin, x.dtype, tuple(x.shape)))
+    Ho, Wo = conv.out_size(H, W)
+    M = B * Ho * Wo
+    cap = workspace.numel() // conv.row_bytes() // 128 * 128
+    rows = cap if chunk_rows is None else int(chunk_rows)
+    if rows < 128 or rows % 128 or rows > cap:
+        raise ValueError("conv2d: chunks of %d rows (a multiple of 128, at most %d for this workspace)" % (rows, cap))
+    if out is None:
+        out = torch.empty((B, Ho, Wo, conv.cout), dtype=torch.float32, device=x.device)
+    lib = _lib.load()
+    with torch.cuda.device(x.device):
+        for r0 in range(0, M, rows):
+            n = min(rows, M - r0)
+            check(lib.sr_conv_pack(_p(x), B, H, W, Cin, conv.kh, conv.kw, conv.stride, conv.pad, int(conv.reflect),
+                                   int(conv.transposed), Ho, Wo, r0, n, _p(workspace), _stream()), "conv_pack")
+            dst = C.c_void_p(out.data_ptr() + r0 * conv.cout * 4)
+            check(lib.sr_tc_linear(_p(workspace), _p(conv.W), _p(conv.bias), n, conv.cout, conv.K, conv.cout, int(act),
+                                   1, None, 0, 1.0, None, 0, 0, dst, conv.cout, 0, conv.cout, None, None, 0, 0, 1.0,
+                                   None, _stream()), "tc_linear")
+    return out
+
+
+def instance_norm_stats(y):
+    """y fp32 [B,H,W,C] -> (mean, rstd) fp32 [B,C]: InstanceNorm2d's per-instance statistics (biased variance, eps
+    1e-5), deterministic and independent of B."""
+    _need_cuda(y)
+    B, C_ = int(y.shape[0]), int(y.shape[-1])
+    HW = y.numel() // (B * C_)
+    lib = _lib.load()
+    part = torch.empty((lib.sr_instance_norm_partial_bytes(B, HW, C_),), dtype=torch.uint8, device=y.device)
+    mean = torch.empty((B, C_), dtype=torch.float32, device=y.device)
+    rstd = torch.empty((B, C_), dtype=torch.float32, device=y.device)
+    with torch.cuda.device(y.device):
+        check(lib.sr_instance_norm_stats(_p(y), B, HW, C_, _p(part), _p(mean), _p(rstd), _stream()),
+              "instance_norm_stats")
+    return mean, rstd
+
+
+def instance_norm_apply(y, mean, rstd, residual=None, relu=False, out=None):
+    """out = relu?((y - mean) * rstd) (+ residual), all fp32 [B,H,W,C] (out may be y or residual)."""
+    _need_cuda(y, mean, rstd, residual)
+    B, C_ = int(y.shape[0]), int(y.shape[-1])
+    if residual is not None and residual.shape != y.shape:
+        raise ValueError("instance_norm_apply: residual %s, y %s" % (tuple(residual.shape), tuple(y.shape)))
+    out = torch.empty_like(y) if out is None else out
+    with torch.cuda.device(y.device):
+        check(_lib.load().sr_instance_norm_apply(_p(y), B, y.numel() // (B * C_), C_, _p(mean), _p(rstd),
+                                                 _p(residual), int(bool(relu)), _p(out), _stream()),
+              "instance_norm_apply")
+    return out
+
+
+def normal_unwarp(net_out, boxes, fg, H, W):
+    """net_out fp32 [B,S,S,3] (channels-last tanh output), boxes fp32 [B,4] (x, y, w, h), fg uint8 [B,H,W] (nonzero =
+    foreground) or None -> uint8 BGR [B,H,W,3]: generate_normals.py:149-165 (grid_sample back onto the frame, zero
+    where |n| < 1e-4 or background, (n*0.5 + 0.5)[::-1]*255 truncated)."""
+    _need_cuda(net_out, boxes, fg)
+    B, S = int(net_out.shape[0]), int(net_out.shape[1])
+    if tuple(net_out.shape) != (B, S, S, 3) or tuple(boxes.shape) != (B, 4) or \
+            (fg is not None and tuple(fg.shape) != (B, H, W)):
+        raise ValueError("normal_unwarp: net_out [B,S,S,3], boxes [B,4], fg [B,H,W] expected")
+    out = torch.empty((B, H, W, 3), dtype=torch.uint8, device=net_out.device)
+    with torch.cuda.device(net_out.device):
+        check(_lib.load().sr_normal_unwarp(_p(net_out.contiguous()), B, S, _p(boxes.float().contiguous()),
+                                           _p(fg.contiguous() if fg is not None else None), int(H), int(W), _p(out),
+                                           _stream()), "normal_unwarp")
+    return out
