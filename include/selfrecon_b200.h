@@ -422,6 +422,60 @@ int sr_texture_finish(int64_t T, int S, const int64_t* texel_index, const float*
                       const int32_t* slot_view, float c0, int min_views, float* tex_median, uint8_t* mask_final,
                       int32_t* view_id, int32_t* count, cudaStream_t s);
 
+/* Template simplification: one round of parallel quadric edge collapse (uvmap.simplify; the rules are in
+ * csrc/mesh_simplify.cu).  verts [V,3] float, faces [F,3] int64 with every index in [0, V); edges [E,2] (a < b),
+ * nbr_off [V+1] / nbr = the edge table and directed neighbour CSR of sr_mesh_reg_topology; vf_off [V+1] / vf = each
+ * vertex's faces, ascending.
+ *   sr_simplify_quadrics: Q [V,10] (upper triangle of the 4x4 plane quadric, row-major), fixed [V] (0/1).
+ *   sr_simplify_edge_cost: vstar [E,3], cost [E] (fp64), key [E] = (bits of (float)cost << 32) | e for a valid edge,
+ *     else ~0.  E < 2^32.
+ *   sr_simplify_select: m1 / m2 [V] work, sel [E] (0/1) = the edges whose key is the minimum over both endpoints' two
+ *     rings.  Integer atomicMin only.
+ *   sr_simplify_collapse: remap [V] (b -> a for a selected (a, b), else v), pos [V,3] (fp32(v*) at a), face_alive [F],
+ *     vert_alive [V].
+ *   sr_simplify_compact: face_cum / vert_cum = inclusive prefix sums of the alive flags; out_verts [V',3] and
+ *     out_faces [F',3] keep the survivors in ascending order. */
+int sr_simplify_quadrics(const float* verts, const int64_t* faces, int64_t V, int64_t F, const int64_t* vf_off,
+                         const int64_t* vf, const int64_t* nbr_off, const int64_t* nbr, double* Q, uint8_t* fixed,
+                         cudaStream_t s);
+int sr_simplify_edge_cost(const float* verts, const int64_t* faces, const int64_t* edges, int64_t E,
+                          const int64_t* vf_off, const int64_t* vf, const int64_t* nbr_off, const int64_t* nbr,
+                          const double* Q, const uint8_t* fixed, double* vstar, double* cost, uint64_t* key,
+                          cudaStream_t s);
+int sr_simplify_select(const int64_t* edges, int64_t E, int64_t V, const int64_t* nbr_off, const int64_t* nbr,
+                       const uint64_t* key, uint64_t* m1, uint64_t* m2, uint8_t* sel, cudaStream_t s);
+int sr_simplify_collapse(const float* verts, const int64_t* faces, int64_t V, int64_t F, const int64_t* edges,
+                         int64_t E, const uint8_t* sel, const double* vstar, int64_t* remap, float* pos,
+                         uint8_t* face_alive, uint8_t* vert_alive, cudaStream_t s);
+int sr_simplify_compact(const int64_t* faces, int64_t V, int64_t F, const int64_t* remap, const float* pos,
+                        const uint8_t* face_alive, const uint8_t* vert_alive, const int64_t* face_cum,
+                        const int64_t* vert_cum, float* out_verts, int64_t* out_faces, cudaStream_t s);
+
+/* UV atlas of a template mesh (uvmap.unwrap; the rules are in csrc/uv_atlas.cu).  faces [F,3] int64, vf_off / vf as
+ * above.
+ *   sr_uv_face_adjacency: adj [F,3] = the face across the edge opposite each corner when it has two faces, else -1.
+ *   sr_uv_labels: normal [F,3] unit (0 at zero area), area [F] (fp64), label [F] in [0, 26) after `passes` smoothing
+ *     passes (work [F] is the ping-pong buffer); 35 <= max_angle <= 80 degrees.
+ *   sr_uv_chart_hook: one in-place hooking pass over cid [F] (start: cid = f); changed = 1 when an id moved.  Repeat
+ *     until changed = 0: cid = the minimum face id of the chart.
+ *   sr_uv_chart_project: C charts, chart_off [C+1] into uv_vert [T] (the vertex of each (chart, vertex) UV vertex,
+ *     grouped by chart), chart_label [C] -> uvl [T,2] chart-local coordinates (3-D units, minimum 0) and box [C,2].
+ *   sr_uv_place: vt [T,2] = (float)(offset[uv_chart] + scale * uvl).
+ *   sr_uv_coverage: count [R,R] = the number of UV faces covering each texel centre (row 0 = v near 1); bad [F] (may
+ *     be NULL) = 1 for a face covering a texel counted more than once. */
+int sr_uv_face_adjacency(const int64_t* faces, int64_t F, const int64_t* vf_off, const int64_t* vf, int64_t* adj,
+                         cudaStream_t s);
+int sr_uv_labels(const float* verts, const int64_t* faces, int64_t F, const int64_t* adj, float max_angle, int passes,
+                 double* normal, double* area, int32_t* label, int32_t* work, cudaStream_t s);
+int sr_uv_chart_hook(const int64_t* adj, const int32_t* label, int64_t F, int64_t* cid, int32_t* changed,
+                     cudaStream_t s);
+int sr_uv_chart_project(const float* verts, int64_t C, const int64_t* chart_off, const int64_t* uv_vert,
+                        const int32_t* chart_label, double* uvl, double* box, cudaStream_t s);
+int sr_uv_place(const double* uvl, const int64_t* uv_chart, int64_t T, const double* offset, double scale, float* vt,
+                cudaStream_t s);
+int sr_uv_coverage(const float* vt, const int64_t* ft, int64_t F, int R, int32_t* count, uint8_t* bad,
+                   cudaStream_t s);
+
 /* Skin-weight volume of a new sequence (model/Deformer.py:235-284, utils/LBSWsmpl.py:2-52: compute_lbswField and
  * smooth_weights).  Volumes are [C][D][H][W] float (x fastest), (W, H, D) = the resolutions; bmin / bmax are HOST [3].
  *   sr_lbsw_knn_blend: verts [V,3], vert_ws [V,C].  Voxel (i, j, l) has the centre u * (hi - lo) + lo with

@@ -133,6 +133,17 @@ SIGNATURES = {
     "sr_texture_accumulate": (C.c_int, [i64, i32, c_f, c_f, c_f, c_f, i64, i64, c_f, c_f, c_f, i32, i32, i32, c_f, c_f,
                                         c_f, c_f, c_f, stream_t]),
     "sr_texture_finish": (C.c_int, [i64, i32, c_f, c_f, c_f, c_f, f32, i32, c_f, c_f, c_f, c_f, stream_t]),
+    "sr_simplify_quadrics": (C.c_int, [c_f, c_f, i64, i64, c_f, c_f, c_f, c_f, c_f, c_f, stream_t]),
+    "sr_simplify_edge_cost": (C.c_int, [c_f, c_f, c_f, i64, c_f, c_f, c_f, c_f, c_f, c_f, c_f, c_f, c_f, stream_t]),
+    "sr_simplify_select": (C.c_int, [c_f, i64, i64, c_f, c_f, c_f, c_f, c_f, c_f, stream_t]),
+    "sr_simplify_collapse": (C.c_int, [c_f, c_f, i64, i64, c_f, i64, c_f, c_f, c_f, c_f, c_f, c_f, stream_t]),
+    "sr_simplify_compact": (C.c_int, [c_f, i64, i64, c_f, c_f, c_f, c_f, c_f, c_f, c_f, c_f, stream_t]),
+    "sr_uv_face_adjacency": (C.c_int, [c_f, i64, c_f, c_f, c_f, stream_t]),
+    "sr_uv_labels": (C.c_int, [c_f, c_f, i64, c_f, f32, i32, c_f, c_f, c_f, c_f, stream_t]),
+    "sr_uv_chart_hook": (C.c_int, [c_f, c_f, i64, c_f, c_f, stream_t]),
+    "sr_uv_chart_project": (C.c_int, [c_f, i64, c_f, c_f, c_f, c_f, c_f, stream_t]),
+    "sr_uv_place": (C.c_int, [c_f, c_f, i64, c_f, C.c_double, c_f, stream_t]),
+    "sr_uv_coverage": (C.c_int, [c_f, c_f, i64, i32, c_f, c_f, stream_t]),
     "sr_lbsw_knn_blend": (C.c_int, [c_f, c_f, i32, i32, C.POINTER(f32), C.POINTER(f32), i32, i32, i32, i32, i32, c_f,
                                     c_f, stream_t]),
     "sr_lbsw_smooth_pass": (C.c_int, [c_f, c_f, i32, i32, i32, i32, f32, stream_t]),

@@ -324,6 +324,158 @@ _KERNELS_PER_CALL.update({"mesh_reg_edge_keys": 1, "mesh_reg_edge_runs": 1, "mes
                           "mesh_reg_forward": 2, "mesh_reg_backward": 1})
 
 
+def simplify_quadrics(verts, faces, csr, topo):
+    """One simplification round's vertex pass (csrc/mesh_simplify.cu): verts [V,3] float32, faces [F,3] int64, csr =
+    (offsets, face ids) of each vertex's faces, topo = mesh_reg_topology(faces, V) -> (Q [V,10] float64, fixed [V]
+    uint8)."""
+    _need_cuda(verts, faces, csr[0], csr[1])
+    V, F = verts.shape[0], faces.shape[0]
+    Q = torch.empty((V, 10), dtype=torch.float64, device=verts.device)
+    fixed = torch.empty(V, dtype=torch.uint8, device=verts.device)
+    with torch.cuda.device(verts.device):
+        check(_lib.load().sr_simplify_quadrics(_p(verts), _p(faces), V, F, _p(csr[0]), _p(csr[1]), _p(topo.nbr_off),
+                                               _p(topo.nbr), _p(Q), _p(fixed), _stream()), "simplify_quadrics")
+    return Q, fixed
+
+
+def simplify_edge_cost(verts, faces, csr, topo, Q, fixed):
+    """-> (vstar [E,3] float64, cost [E] float64, key [E] int64 holding the uint64 keys: ~0 = -1 for an edge that may
+    not collapse) of the edges topo.edges."""
+    _need_cuda(verts, faces, Q, fixed)
+    E, dev = topo.E, verts.device
+    vstar = torch.empty((E, 3), dtype=torch.float64, device=dev)
+    cost = torch.empty(E, dtype=torch.float64, device=dev)
+    key = torch.empty(E, dtype=torch.int64, device=dev)
+    with torch.cuda.device(dev):
+        check(_lib.load().sr_simplify_edge_cost(_p(verts), _p(faces), _p(topo.edges), E, _p(csr[0]), _p(csr[1]),
+                                                _p(topo.nbr_off), _p(topo.nbr), _p(Q), _p(fixed), _p(vstar), _p(cost),
+                                                _p(key), _stream()), "simplify_edge_cost")
+    return vstar, cost, key
+
+
+def simplify_select(topo, key):
+    """-> sel [E] uint8: the edges whose key is the minimum over the two rings of both endpoints."""
+    _need_cuda(key)
+    dev = key.device
+    m1 = torch.empty(topo.V, dtype=torch.int64, device=dev)
+    m2 = torch.empty_like(m1)
+    sel = torch.empty(topo.E, dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+        check(_lib.load().sr_simplify_select(_p(topo.edges), topo.E, topo.V, _p(topo.nbr_off), _p(topo.nbr), _p(key),
+                                             _p(m1), _p(m2), _p(sel), _stream()), "simplify_select")
+    return sel
+
+
+def simplify_collapse(verts, faces, edges, sel, vstar, n_verts, n_faces):
+    """Collapses the selected edges (each removes one vertex and two faces) -> (verts [n_verts,3], faces [n_faces,3]),
+    survivors in ascending order.  n_verts / n_faces are the counts the caller derived from its selection."""
+    _need_cuda(verts, faces, edges, sel, vstar)
+    V, F, E, dev = verts.shape[0], faces.shape[0], edges.shape[0], verts.device
+    lib = _lib.load()
+    remap = torch.empty(V, dtype=torch.int64, device=dev)
+    pos = torch.empty_like(verts)
+    face_alive = torch.empty(F, dtype=torch.uint8, device=dev)
+    vert_alive = torch.empty(V, dtype=torch.uint8, device=dev)
+    out_v = torch.empty((n_verts, 3), dtype=torch.float32, device=dev)
+    out_f = torch.empty((n_faces, 3), dtype=torch.int64, device=dev)
+    with torch.cuda.device(dev):
+        check(lib.sr_simplify_collapse(_p(verts), _p(faces), V, F, _p(edges), E, _p(sel), _p(vstar), _p(remap),
+                                       _p(pos), _p(face_alive), _p(vert_alive), _stream()), "simplify_collapse")
+        face_cum, vert_cum = torch.cumsum(face_alive, 0), torch.cumsum(vert_alive, 0)
+        check(lib.sr_simplify_compact(_p(faces), V, F, _p(remap), _p(pos), _p(face_alive), _p(vert_alive),
+                                      _p(face_cum), _p(vert_cum), _p(out_v), _p(out_f), _stream()), "simplify_compact")
+    return out_v, out_f
+
+
+_KERNELS_PER_CALL.update({"simplify_select": 3, "simplify_collapse": 3})
+
+
+def uv_face_adjacency(faces, csr):
+    """faces [F,3] int64, csr = vertex -> face CSR -> adj [F,3] int64 (the face across each corner's opposite edge
+    when that edge has two faces, else -1)."""
+    _need_cuda(faces, csr[0], csr[1])
+    F = faces.shape[0]
+    adj = torch.empty((F, 3), dtype=torch.int64, device=faces.device)
+    with torch.cuda.device(faces.device):
+        check(_lib.load().sr_uv_face_adjacency(_p(faces), F, _p(csr[0]), _p(csr[1]), _p(adj), _stream()),
+              "uv_face_adjacency")
+    return adj
+
+
+UV_DIRECTIONS = 26
+
+
+def uv_labels(verts, faces, adj, max_angle, passes=8):
+    """-> (unit normals [F,3] float64, areas [F] float64, labels [F] int32 in [0, 26)) after `passes` smoothing
+    passes."""
+    _need_cuda(verts, faces, adj)
+    F, dev = faces.shape[0], verts.device
+    normal = torch.empty((F, 3), dtype=torch.float64, device=dev)
+    area = torch.empty(F, dtype=torch.float64, device=dev)
+    label = torch.empty(F, dtype=torch.int32, device=dev)
+    work = torch.empty_like(label)
+    with torch.cuda.device(dev):
+        check(_lib.load().sr_uv_labels(_p(verts), _p(faces), F, _p(adj), float(max_angle), int(passes), _p(normal),
+                                       _p(area), _p(label), _p(work), _stream()), "uv_labels")
+    return normal, area, label
+
+
+_KERNELS_PER_CALL["uv_labels"] = 9
+
+
+def uv_chart_ids(adj, label, check_every=8):
+    """-> cid [F] int64 = the minimum face id of each face's chart (same-label faces joined across two-face edges).
+    Hooking passes run in groups of check_every between readbacks of the changed flag."""
+    _need_cuda(adj, label)
+    F, dev = label.shape[0], label.device
+    cid = torch.arange(F, dtype=torch.int64, device=dev)
+    changed = torch.empty(1, dtype=torch.int32, device=dev)
+    flags = torch.empty(check_every, dtype=torch.int32, device=dev)
+    lib = _lib.load()
+    with torch.cuda.device(dev):
+        while True:
+            for i in range(check_every):
+                check(lib.sr_uv_chart_hook(_p(adj), _p(label), F, _p(cid), _p(changed), _stream()), "uv_chart_hook")
+                flags[i:i + 1].copy_(changed)
+            if not bool(flags[-1]):
+                return cid
+
+
+def uv_chart_project(verts, chart_off, uv_vert, chart_label):
+    """-> (uvl [T,2] float64 chart-local coordinates, box [C,2] float64 chart extents) of the UV vertices uv_vert [T]
+    grouped by chart (chart_off [C+1]), projected along the directions chart_label [C] int32."""
+    _need_cuda(verts, chart_off, uv_vert, chart_label)
+    C, T, dev = chart_label.shape[0], uv_vert.shape[0], verts.device
+    uvl = torch.empty((T, 2), dtype=torch.float64, device=dev)
+    box = torch.empty((C, 2), dtype=torch.float64, device=dev)
+    with torch.cuda.device(dev):
+        check(_lib.load().sr_uv_chart_project(_p(verts), C, _p(chart_off), _p(uv_vert), _p(chart_label), _p(uvl),
+                                              _p(box), _stream()), "uv_chart_project")
+    return uvl, box
+
+
+def uv_place(uvl, uv_chart, offset, scale):
+    """-> vt [T,2] float32 = offset[uv_chart] + scale * uvl."""
+    _need_cuda(uvl, uv_chart, offset)
+    T = uvl.shape[0]
+    vt = torch.empty((T, 2), dtype=torch.float32, device=uvl.device)
+    with torch.cuda.device(uvl.device):
+        check(_lib.load().sr_uv_place(_p(uvl), _p(uv_chart), T, _p(offset), float(scale), _p(vt), _stream()),
+              "uv_place")
+    return vt
+
+
+def uv_coverage(vt, ft, R, want_bad=True):
+    """-> (count [R,R] int32 UV faces per texel centre, bad [F] uint8 faces on a texel counted twice, or None)."""
+    _need_cuda(vt, ft)
+    F, dev = ft.shape[0], vt.device
+    count = torch.empty((R, R), dtype=torch.int32, device=dev)
+    bad = torch.empty(F, dtype=torch.uint8, device=dev) if want_bad else None
+    with torch.cuda.device(dev):
+        check(_lib.load().sr_uv_coverage(_p(vt), _p(ft), F, int(R), _p(count), _p(bad), _stream()), "uv_coverage")
+    return count, bad
+
+
 TEXTURE_MAX_SLOTS = 64     # SR_TEXTURE_MAX_SLOTS
 
 
