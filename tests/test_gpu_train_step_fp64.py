@@ -2,7 +2,7 @@
 (train_step_twin.py), one step per term with only that weight positive: eikonal (grad_weight), offset, def_regu,
 colour, weighted normal, and the mix of the shipped coarse level's ray weights.  The colour and normal terms run the
 surface-point branch and with it the implicit term of propagateTmpPsGrad.  The template (point-cloud silhouette and
-mesh) term is not covered here.
+mesh) term of forward() is pinned to the same twin by test_gpu_train_template_fp64.py.
 
 Per term: the loss value (relative), dL/dTmpPs, and each parameter group's gradient as ||g - g64|| / ||g64|| (SDF,
 translator, renderer, poses, translations, latent codes), once for the gradient of loss.backward() (the direct part)
