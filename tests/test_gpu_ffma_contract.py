@@ -516,37 +516,49 @@ CAM = (0.0, 0.2, -3.0)
 ATHR = 3.0
 
 
-def _trace_setup(pair, dev, n=320):
-    s_name, d_name, with_lbs = TRACE_PAIRS[pair]
+def _trace_setup(pair, dev, n=320, odev="cpu"):
+    """pair: a TRACE_PAIRS name or its (sdf, translator or None, with LBS) triple.  The float64 oracle's inputs and
+    functions live on `odev`."""
+    s_name, d_name, with_lbs = TRACE_PAIRS[pair] if isinstance(pair, str) else pair
     sdf = sdf_net(s_name, dev)
     dnet = translator_net(d_name, dev) if d_name else None
     st, lref = lbs_setup(dev) if with_lbs else (None, None)
     cd = conds(dev)
-    x0 = _sample(n, 600, -0.7, 0.7).double()
-    bi = torch.randint(0, NFRAMES, (n,), generator=torch.Generator().manual_seed(6))
-    cam = torch.tensor(CAM, dtype=torch.float64)
-    lcpu = {k: v.cpu() for k, v in lref.items()} if lref is not None else None
+    x0 = _sample(n, 600, -0.7, 0.7).double().to(odev)
+    bi = torch.randint(0, NFRAMES, (n,), generator=torch.Generator().manual_seed(6)).to(odev)
+    cam = torch.tensor(CAM, dtype=torch.float64, device=odev)
+    lo = {k: v.to(odev) for k, v in lref.items()} if lref is not None else None
 
     def sdf_fn(p):
         return R.mlp(sdf.layers, R.embed(p, sdf.multires, sdf.pe_w), sdf.d_in)[:, :1]
 
     def def_fn(p, b):
-        if dnet is None:
-            return p
-        p1 = p + R.translator_offset(dnet.layers, p, 6, dnet.pe_w, cd.cpu(), b)
-        return p1 if lcpu is None else O.lbs_forward(lcpu["ws"], lcpu["bmin"], lcpu["bmax"], lcpu["A"],
-                                                     lcpu["trans"], p1, b)
+        p1 = p if dnet is None else p + R.translator_offset(dnet.layers, p, 6, dnet.pe_w, cd.to(odev), b)
+        return p1 if lo is None else O.lbs_forward(lo["ws"], lo["bmin"], lo["bmax"], lo["A"], lo["trans"], p1, b)
     with torch.no_grad():
-        miss = 0.03 * torch.randn(n, 3, generator=torch.Generator().manual_seed(7), dtype=torch.float64)
+        miss = 0.03 * torch.randn(n, 3, generator=torch.Generator().manual_seed(7), dtype=torch.float64).to(odev)
         rays = torch.nn.functional.normalize(def_fn(x0, bi) + miss - cam, dim=1)
         f0 = sdf_fn(x0).view(-1).abs()
     return sdf, dnet, st, cd, x0, bi, cam, rays, f0, sdf_fn, def_fn
 
 
-def _oracle_trace(cam, rays, x0, bi, sdf_fn, def_fn, dth, times):
-    sens = dict(eps_f=1e-5, eps_a=1e-3)
-    p, conv, _ = O.optimize_surface_ps(cam, rays, x0, bi, sdf_fn, def_fn, dth, ATHR, 3.05, 1.0, times, sensitivity=sens)
-    return p, conv, sens["sensitive"]
+def _oracle_trace(cam, rays, x0, bi, sdf_fn, def_fn, dth, times, eps=(1e-5, 1e-3), with_iters=False):
+    """eps: the engine's error bounds on f and on the angle (degrees) that mark a ray decision-sensitive; with_iters
+    also returns how many times each ray was updated."""
+    sens = dict(eps_f=eps[0], eps_a=eps[1])
+    p, conv, iters = O.optimize_surface_ps(cam, rays, x0, bi, sdf_fn, def_fn, dth, ATHR, 3.05, 1.0, times,
+                                           sensitivity=sens)
+    return (p, conv, sens["sensitive"], iters) if with_iters else (p, conv, sens["sensitive"])
+
+
+def _split_threshold(cam, rays, x0, bi, sdf_fn, def_fn, f0):
+    """A dthreshold that leaves 20-80 % of the rays unconverged after one and after two iterations."""
+    for q in (0.3, 0.2, 0.12, 0.06, 0.03, 0.015, 0.007, 0.003, 0.001):
+        cand = float(f0.quantile(q))
+        fr = [float(_oracle_trace(cam, rays, x0, bi, sdf_fn, def_fn, cand, t)[1].float().mean()) for t in (1, 2)]
+        if all(0.2 <= v <= 0.8 for v in fr):
+            return cand
+    raise AssertionError("no threshold splits the rays")
 
 
 @pytest.mark.parametrize("pair", list(TRACE_PAIRS))
@@ -554,15 +566,7 @@ def test_trace_matches_fp64_oracle(cuda_dev, pair):
     from selfreconcode_b200 import ops
     sdf, dnet, st, cd, x0, bi, cam, rays, f0, sdf_fn, def_fn = _trace_setup(pair, cuda_dev)
     n = x0.shape[0]
-    # a threshold that leaves 20-80 % of the rays unconverged after one and after two iterations
-    dth = None
-    for q in (0.3, 0.2, 0.12, 0.06, 0.03, 0.015, 0.007, 0.003, 0.001):
-        cand = float(f0.quantile(q))
-        fr = [float(_oracle_trace(cam, rays, x0, bi, sdf_fn, def_fn, cand, t)[1].float().mean()) for t in (1, 2)]
-        if all(0.2 <= v <= 0.8 for v in fr):
-            dth = cand
-            break
-    assert dth is not None, "no threshold splits the rays"
+    dth = _split_threshold(cam, rays, x0, bi, sdf_fn, def_fn, f0)
     for times in (1, 2):
         po, co, sens = _oracle_trace(cam, rays, x0, bi, sdf_fn, def_fn, dth, times)
         res = {mode: ops.trace_surface_points(sdf.fused.truncated_last(1), dnet.fused if dnet else None, st,
