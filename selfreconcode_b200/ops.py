@@ -1646,9 +1646,15 @@ class _TcShadeBuffers:
         self.grad = f32(cap, 3)
 
 
-# one buffer set per (device, SDF widths), grown (by at least a quarter, in steps of 4096 points) when a call brings
-# more points than it holds: a point count that changes from frame to frame keeps hitting it
+# one buffer set per (device, SDF layer shapes), grown (by at least a quarter, in steps of 4096 points) when a call
+# brings more points than it holds: a point count that changes from frame to frame keeps hitting it
 _tc_shade_bufs = {}
+
+
+def _tc_shade_key(dev, d):
+    """The buffer set's key: every size _TcShadeBuffers reads from the descriptor.  The activation tiles are sized by
+    each layer's input width k, which the output widths n and d_in do not fix (a skip layer's k is n + d_in)."""
+    return (dev.index, tuple((d.layer[i].n, d.layer[i].k) for i in range(d.n_layers)), d.d_in)
 
 
 def _sdf_grad_tc(lib, sdf_full, pts, P):
@@ -1658,7 +1664,7 @@ def _sdf_grad_tc(lib, sdf_full, pts, P):
     encoding's cotangent without the skip layer's part, g_out [P, pad32(d_in)]."""
     dev = pts.device
     d = sdf_full.desc
-    key = (dev.index, tuple(d.layer[i].n for i in range(d.n_layers)), d.d_in)
+    key = _tc_shade_key(dev, d)
     B = _tc_shade_bufs.get(key)
     if B is None or B.cap < P:
         cap = _pad(max(P, B.cap + B.cap // 4 if B is not None else 0), 4096)
@@ -1692,6 +1698,13 @@ def shade_and_render_tc(sdf_full, def_net, lbs, render_net, pts, rays, batch_ind
     pts = pts.detach().contiguous().float()
     rays = rays.detach().contiguous().float()
     bi = batch_inds.contiguous().to(torch.int64) if batch_inds is not None else None
+    if P == 0:
+        # an empty ray set (trace_surface_points returns empty tensors for one): the kernels refuse P = 0
+        rd = render_net.desc
+        e3 = lambda: torch.empty((0, 3), dtype=torch.float32, device=dev)   # noqa: E731
+        out = (e3(), e3(), torch.empty((0, rd.layer[rd.n_layers - 1].n), dtype=torch.float32, device=dev), e3(),
+               torch.empty((0,), dtype=torch.bool, device=dev))
+        return out + (e3(),) if deformed_normals else out
     lib = _lib.load()
     with torch.cuda.device(dev):
         if TC_DUAL_STREAM and def_net is not None:

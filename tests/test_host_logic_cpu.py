@@ -75,3 +75,38 @@ def test_bench_parity_report_counts():
     assert rep["sign_mismatch"] == 2 and rep["sign_mismatch_outside_fp32_band"] == 1
     assert rep["queried_set_mismatch"] == 0 and rep["mc_mesh_identical"] is True
     assert rep["mc_on_oracle_grid_faces_identical"] is False and rep["mc_on_oracle_grid_verts_identical"] is True
+
+
+def test_tc_shade_buffer_key_fixes_every_size():
+    """ops._sdf_grad_tc keeps one _TcShadeBuffers set per key and reuses it for every network with that key, so the key
+    must fix every size the set is built from: the embedded input's width, each layer's n (staging tiles, outputs) and
+    each layer's k (the kept activation tiles).  Two production-shaped SDFs whose skip layer sits at different depths
+    have the same widths n and d_in but different k's."""
+    from selfreconcode_b200 import ops
+
+    def desc(ns, skip_at, d_in=39):
+        d = _lib.MlpDesc()
+        d.n_layers, d.d_in = len(ns), d_in
+        for i, n in enumerate(ns):
+            ly = d.layer[i]
+            ly.n, ly.skip = n, int(i == skip_at)
+            ly.k = (ns[i - 1] if i else d_in) + (d_in if i == skip_at else 0)
+        return d
+
+    def sizes(d):
+        """What _TcShadeBuffers reads from the descriptor (its buffer widths, in columns)."""
+        pad = lambda x: (x + 31) // 32 * 32                    # noqa: E731
+        return (pad(d.d_in), tuple(pad(d.layer[i + 1].k) for i in range(d.n_layers - 1)), d.layer[d.n_layers - 1].n,
+                max([32] + [pad(d.layer[i].n) for i in range(d.n_layers - 1)]))
+
+    ns = [512] * 3 + [473] + [512] * 4 + [257]
+    descs = [desc(ns, 4), desc(ns, 3), desc(ns, 5), desc(ns, -1), desc([512] * 8 + [1], 4), desc(ns, 4, d_in=51)]
+    dev = torch.device("cuda", 0)
+    seen = {}
+    for d in descs:
+        key = ops._tc_shade_key(dev, d)
+        assert seen.setdefault(key, sizes(d)) == sizes(d), "one key, two buffer layouts"
+    assert len(seen) == len(descs)
+    # widths alone would not tell the skip positions apart (their k's differ)
+    assert len({(tuple(d.layer[i].n for i in range(d.n_layers)), d.d_in) for d in descs[:4]}) == 1
+    assert len({sizes(d) for d in descs[:4]}) == 4
