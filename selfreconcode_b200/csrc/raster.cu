@@ -25,16 +25,28 @@ __device__ __forceinline__ bool load_tri(const float* __restrict__ vs, const lon
   t.x0 = p[a * 3]; t.y0 = p[a * 3 + 1]; t.z0 = p[a * 3 + 2];
   t.x1 = p[b * 3]; t.y1 = p[b * 3 + 1]; t.z1 = p[b * 3 + 2];
   t.x2 = p[c * 3]; t.y2 = p[c * 3 + 1]; t.z2 = p[c * 3 + 2];
-  return t.z0 > 1e-8f && t.z1 > 1e-8f && t.z2 > 1e-8f;
+  // a non-finite vertex drops the face: with z = inf its q_i would be 0 and the face would still cover pixels
+  const bool finite = isfinite(t.x0) && isfinite(t.y0) && isfinite(t.z0) && isfinite(t.x1) && isfinite(t.y1) &&
+                      isfinite(t.z1) && isfinite(t.x2) && isfinite(t.y2) && isfinite(t.z2);
+  return finite && t.z0 > 1e-8f && t.z1 > 1e-8f && t.z2 > 1e-8f;
+}
+
+// Edge function of the directed edge a -> b at (px, py): (xa - px)(yb - py) - (xb - px)(ya - py), twice the signed
+// area of (a, b, p).  Every difference and product is rounded on its own: __fmul_rn / __fsub_rn are never contracted
+// into an FFMA, so edge(a, b) == -edge(b, a) bit for bit.  Two faces sharing an edge then cannot both reject a pixel
+// centre on it (the coverage test is watertight), a face's coverage does not depend on its winding, and the face and
+// resolve kernels take the same decision on the same pixel.  It is also the face area: area = edge(v1, v2) at v0.
+__device__ __forceinline__ float edge_fn(float xa, float ya, float xb, float yb, float px, float py) {
+  return __fsub_rn(__fmul_rn(__fsub_rn(xa, px), __fsub_rn(yb, py)), __fmul_rn(__fsub_rn(xb, px), __fsub_rn(ya, py)));
 }
 
 // barycentrics of pixel centre (px, py); returns false when outside or degenerate
 __device__ __forceinline__ bool bary_at(const Tri& t, float px, float py, float b[3], float& z) {
-  const float area = (t.x1 - t.x0) * (t.y2 - t.y0) - (t.x2 - t.x0) * (t.y1 - t.y0);
+  const float area = edge_fn(t.x1, t.y1, t.x2, t.y2, t.x0, t.y0);
   if (fabsf(area) < 1e-12f) return false;
-  const float w0 = (t.x1 - px) * (t.y2 - py) - (t.x2 - px) * (t.y1 - py);
-  const float w1 = (t.x2 - px) * (t.y0 - py) - (t.x0 - px) * (t.y2 - py);
-  const float w2 = (t.x0 - px) * (t.y1 - py) - (t.x1 - px) * (t.y0 - py);
+  const float w0 = edge_fn(t.x1, t.y1, t.x2, t.y2, px, py);
+  const float w1 = edge_fn(t.x2, t.y2, t.x0, t.y0, px, py);
+  const float w2 = edge_fn(t.x0, t.y0, t.x1, t.y1, px, py);
   const float inv = 1.0f / area;
   const float l0 = w0 * inv, l1 = w1 * inv, l2 = w2 * inv;
   if (l0 < 0.f || l1 < 0.f || l2 < 0.f) return false;

@@ -92,6 +92,11 @@ def raster_mesh(verts_screen, faces, H, W):
     N, V, _ = vs.shape
     F = fc.shape[0]
     dev = vs.device
+    if N == 0 or F == 0:
+        # no frame, or a mesh without faces: every pixel is background (the kernels refuse empty inputs)
+        return (torch.full((N, H, W, 1), -1, dtype=torch.int64, device=dev),
+                torch.full((N, H, W, 1, 3), -1., dtype=torch.float32, device=dev),
+                torch.full((N, H, W, 1), -1., dtype=torch.float32, device=dev))
     keys = torch.empty((N, H, W), dtype=torch.int64, device=dev)
     p2f = torch.empty((N, H, W, 1), dtype=torch.int64, device=dev)
     bary = torch.empty((N, H, W, 1, 3), dtype=torch.float32, device=dev)
