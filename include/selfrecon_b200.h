@@ -422,6 +422,26 @@ int sr_texture_finish(int64_t T, int S, const int64_t* texel_index, const float*
                       const int32_t* slot_view, float c0, int min_views, float* tex_median, uint8_t* mask_final,
                       int32_t* view_id, int32_t* count, cudaStream_t s);
 
+/* Textured rendering of the avatar (selfreconcode_b200.avatar): the baked atlas through a mip pyramid onto the
+ * fragments sr_raster_mesh writes.  Unlit: the atlas already holds the captured shading.
+ *   sr_texture_mips: texture [Ht,Wt,3] uint8 (its own channel order), coverage [Ht,Wt] uint8 -> mips = every level as
+ *     float4 (r, g, b, w), level after level, row-major (16-byte aligned).  Level 0 = (c / 255, w = coverage != 0);
+ *     W_{l+1} = ceil(W_l / 2), H_{l+1} = ceil(H_l / 2) down to 1x1.  A child reduces its (up to) 2x2 parents:
+ *     colour = sum w c / sum w when sum w > 0, else the plain mean of the parents' colours; w = mean of their w.
+ *   sr_shade_textured: pix_to_face [N,H,W] (n*F + f, -1 = empty), bary [N,H,W,3] perspective-correct, verts_screen
+ *     [N,V,3] = (col, row, Z) of mesh n, faces / ft [F,3], vt [T,2].  uv = sum b_i vt[ft[f,i]]; level-l texel
+ *     coordinates (u W_l - 0.5, (1 - v) H_l - 0.5), bilinear with clamp-to-edge; trilinear between floor(lambda) and
+ *     floor(lambda) + 1, lambda = clamp(log2 rho, 0, L - 1), rho = max(|d(u Wt, v Ht)/dcol|, |d(u Wt, v Ht)/drow|) of
+ *     the face's perspective-correct interpolation at the pixel centre (analytic, no neighbour differences).
+ *     out [N,H,W,4] (16-byte aligned): (rgb, 1) on covered pixels, (background, 0) elsewhere; the background is
+ *     bg_image [N,H,W,3] uint8 / 255 when it is not NULL, else bg_color[3] (host array).
+ * One thread owns each output texel / pixel (no atomics: bit-identical reruns). */
+int sr_texture_mips(const uint8_t* texture, const uint8_t* coverage, int Ht, int Wt, float* mips, cudaStream_t s);
+int sr_shade_textured(const int64_t* pix_to_face, const float* bary, int64_t N, int H, int W, const float* verts_screen,
+                      int64_t V, const int64_t* faces, const int64_t* ft, int64_t F, const float* vt, int64_t T,
+                      const float* mips, int Ht, int Wt, const uint8_t* bg_image, const float* bg_color, float* out,
+                      cudaStream_t s);
+
 /* Template simplification: one round of parallel quadric edge collapse (uvmap.simplify; the rules are in
  * csrc/mesh_simplify.cu).  verts [V,3] float, faces [F,3] int64 with every index in [0, V); edges [E,2] (a < b),
  * nbr_off [V+1] / nbr = the edge table and directed neighbour CSR of sr_mesh_reg_topology; vf_off [V+1] / vf = each

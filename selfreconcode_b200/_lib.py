@@ -133,6 +133,9 @@ SIGNATURES = {
     "sr_texture_accumulate": (C.c_int, [i64, i32, c_f, c_f, c_f, c_f, i64, i64, c_f, c_f, c_f, i32, i32, i32, c_f, c_f,
                                         c_f, c_f, c_f, stream_t]),
     "sr_texture_finish": (C.c_int, [i64, i32, c_f, c_f, c_f, c_f, f32, i32, c_f, c_f, c_f, c_f, stream_t]),
+    "sr_texture_mips": (C.c_int, [c_f, c_f, i32, i32, c_f, stream_t]),
+    "sr_shade_textured": (C.c_int, [c_f, c_f, i64, i32, i32, c_f, i64, c_f, c_f, i64, c_f, i64, c_f, i32, i32, c_f,
+                                    C.POINTER(f32), c_f, stream_t]),
     "sr_simplify_quadrics": (C.c_int, [c_f, c_f, i64, i64, c_f, c_f, c_f, c_f, c_f, c_f, stream_t]),
     "sr_simplify_edge_cost": (C.c_int, [c_f, c_f, c_f, i64, c_f, c_f, c_f, c_f, c_f, c_f, c_f, c_f, c_f, stream_t]),
     "sr_simplify_select": (C.c_int, [c_f, i64, i64, c_f, c_f, c_f, c_f, c_f, c_f, stream_t]),

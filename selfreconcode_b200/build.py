@@ -15,7 +15,7 @@ LIBNAME = "libselfrecon_b200.so"
 SOURCES = ["minv3x3.cu", "marching_cubes.cu", "interp2x.cu", "grid_sampler.cu", "mlp_kernels.cu",
            "seg3d.cu", "tc_gemm.cu", "trace_tc.cu", "svals3x3.cu", "tc_wgrad.cu", "raster.cu", "mesh_shade.cu",
            "points_silhouette.cu", "texture_bake.cu", "lbsw_field.cu", "mesh_reg.cu", "frames.cu",
-           "normal_net.cu", "mesh_simplify.cu", "uv_atlas.cu"]
+           "normal_net.cu", "mesh_simplify.cu", "uv_atlas.cu", "avatar_texture.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 

@@ -522,6 +522,89 @@ def texture_finish(texel_index, slots, c0, min_views, n_texels):
     return med, mask, view, count
 
 
+def mip_levels(Ht, Wt):
+    """Level table of sr_texture_mips' pyramid for an Ht x Wt atlas: int64 [L,3] rows (first texel, H_l, W_l), with
+    W_{l+1} = ceil(W_l / 2), H_{l+1} = ceil(H_l / 2) down to 1x1 (host tensor)."""
+    Ht, Wt = int(Ht), int(Wt)
+    if Ht <= 0 or Wt <= 0:
+        raise ValueError("mip_levels: the atlas must not be empty, got %d x %d" % (Ht, Wt))
+    rows, off = [(0, Ht, Wt)], Ht * Wt
+    while Ht > 1 or Wt > 1:
+        Ht, Wt = (Ht + 1) // 2, (Wt + 1) // 2
+        rows.append((off, Ht, Wt))
+        off += Ht * Wt
+    return torch.tensor(rows, dtype=torch.int64)
+
+
+def texture_mips(texture_u8, coverage):
+    """Coverage-weighted mip pyramid of an atlas (csrc/avatar_texture.cu).  texture_u8 [Ht,Wt,3] uint8 in its own
+    channel order, coverage [Ht,Wt] (bool or uint8, nonzero = covered) -> (mips [texels,4] float32 = (r, g, b, w) of
+    every level, levels = mip_levels(Ht, Wt))."""
+    _need_cuda(texture_u8, coverage)
+    if texture_u8.dim() != 3 or texture_u8.shape[2] != 3 or texture_u8.dtype != torch.uint8:
+        raise ValueError("texture_mips: the atlas must be [Ht,Wt,3] uint8, got %s %s"
+                         % (tuple(texture_u8.shape), texture_u8.dtype))
+    Ht, Wt = texture_u8.shape[0], texture_u8.shape[1]
+    if tuple(coverage.shape) != (Ht, Wt) or coverage.dtype not in (torch.bool, torch.uint8):
+        raise ValueError("texture_mips: coverage must be [Ht,Wt] = [%d,%d] bool or uint8" % (Ht, Wt))
+    levels = mip_levels(Ht, Wt)
+    n = int(levels[-1, 0] + levels[-1, 1] * levels[-1, 2])
+    tex = texture_u8.contiguous()
+    cov = coverage.to(torch.uint8).contiguous()
+    mips = torch.empty((n, 4), dtype=torch.float32, device=tex.device)
+    with torch.cuda.device(tex.device):
+        check(_lib.load().sr_texture_mips(_p(tex), _p(cov), int(Ht), int(Wt), _p(mips), _stream()), "texture_mips")
+    global LAUNCHES
+    LAUNCHES += levels.shape[0] - 1        # one launch per level
+    return mips, levels
+
+
+def shade_textured(pix_to_face, bary, verts_screen, faces, ft, vt, mips, levels, background=(1., 1., 1.)):
+    """Unlit trilinear-filtered atlas lookup on rasteriser fragments (csrc/avatar_texture.cu).  pix_to_face
+    [N,H,W(,1)] packed ids n*F + f, bary [N,H,W(,1),3], verts_screen [N,V,3] (col, row, Z), faces / ft [F,3], vt [T,2],
+    (mips, levels) of texture_mips; background = 3 floats or a uint8 image [N,H,W,3] in the atlas' channel order ->
+    images [N,H,W,4]: (rgb, 1) on covered pixels, (background, 0) elsewhere."""
+    bg_img = background if torch.is_tensor(background) else None
+    _need_cuda(pix_to_face, bary, verts_screen, faces, ft, vt, mips, bg_img)
+    vs = verts_screen.detach().contiguous().float()
+    if vs.dim() != 3 or vs.shape[2] != 3:
+        raise ValueError("shade_textured: verts_screen must be [N,V,3]")
+    N, V, _ = vs.shape
+    if pix_to_face.dim() not in (3, 4) or pix_to_face.shape[0] != N:
+        raise ValueError("shade_textured: pix_to_face must be [N,H,W] or [N,H,W,1] with N = %d" % N)
+    H, W = int(pix_to_face.shape[1]), int(pix_to_face.shape[2])
+    p2f = pix_to_face.contiguous().to(torch.int64)
+    br = bary.detach().contiguous().float()
+    fc = faces.contiguous().to(torch.int64)
+    ftc = ft.contiguous().to(torch.int64)
+    vtc = vt.detach().contiguous().float()
+    if p2f.numel() != N * H * W or br.numel() != 3 * N * H * W:
+        raise ValueError("shade_textured: pix_to_face / bary do not match [N,H,W] = [%d,%d,%d]" % (N, H, W))
+    if fc.dim() != 2 or fc.shape[1] != 3 or ftc.shape != fc.shape or vtc.dim() != 2 or vtc.shape[1] != 2:
+        raise ValueError("shade_textured: faces and ft must be [F,3] and vt [T,2]")
+    Ht, Wt = int(levels[0, 1]), int(levels[0, 2])
+    n = int(levels[-1, 0] + levels[-1, 1] * levels[-1, 2])
+    mips = mips.contiguous()
+    if mips.dtype != torch.float32 or tuple(mips.shape) != (n, 4):
+        raise ValueError("shade_textured: mips must be the [%d,4] float32 pyramid of the level table" % n)
+    col = None
+    if bg_img is not None:
+        if bg_img.dtype != torch.uint8 or tuple(bg_img.shape) != (N, H, W, 3):
+            raise ValueError("shade_textured: a background image must be [N,H,W,3] = [%d,%d,%d,3] uint8" % (N, H, W))
+        bg_img = bg_img.contiguous()
+    else:
+        col = (C.c_float * 3)(*[float(c) for c in background])
+    out = torch.empty((N, H, W, 4), dtype=torch.float32, device=vs.device)
+    with torch.cuda.device(vs.device):
+        check(_lib.load().sr_shade_textured(_p(p2f), _p(br), N, H, W, _p(vs), V, _p(fc), _p(ftc), fc.shape[0], _p(vtc),
+                                            vtc.shape[0], _p(mips), Ht, Wt, _p(bg_img), col, _p(out),
+                                            _stream()), "shade_textured")
+    return out
+
+
+_KERNELS_PER_CALL["shade_textured"] = 1
+
+
 LBSW_MAX_K = 32           # SR_LBSW_MAX_K
 LBSW_MAX_C = 32           # SR_LBSW_MAX_C
 

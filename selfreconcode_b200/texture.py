@@ -79,6 +79,15 @@ def _as_device(x, device, dtype=None):
     return t.to(device=device, dtype=dtype if dtype is not None else t.dtype).contiguous()
 
 
+def uv_raster(vt, ft, Ht, Wt):
+    """UV faces on an Ht x Wt atlas: texel (i, j) is the pixel centre (col j, row i) of the screen vertices
+    (u Wt - 0.5, (1-v) Ht - 0.5, 1).  vt [T,2] float32, ft [F,3] int64 device tensors -> (face [Ht,Wt] int64, -1 =
+    uncovered; barycentrics [Ht,Wt,3])."""
+    uv = torch.stack([vt[:, 0] * Wt - 0.5, (1. - vt[:, 1]) * Ht - 0.5, torch.ones_like(vt[:, 0])], dim=-1)
+    p2f, bary, _ = ops.raster_mesh(uv[None], ft, Ht, Wt)
+    return p2f.view(Ht, Wt), bary.view(Ht, Wt, 3)
+
+
 class TextureBaker:
     """Streams frames into an R x R atlas with `views` slots per covered texel.  Device memory: 20 B per slot and
     covered texel (at most views * R^2 * 20 B: 2.8 GB at R = 1680 and 50 slots) plus 36 B per covered texel."""
@@ -101,9 +110,7 @@ class TextureBaker:
         ft = _as_device(ft, self.device, torch.int64).reshape(-1, 3)
         if ft.shape != self.faces.shape:
             raise ValueError("TextureBaker: ft must have one row per face (%d), got %d" % (self.faces.shape[0], ft.shape[0]))
-        # UV raster: texel (i, j) is the pixel centre (col j, row i) of the screen vertices (u R - 0.5, (1-v) R - 0.5, 1)
-        uv = torch.stack([vt[:, 0] * R - 0.5, (1. - vt[:, 1]) * R - 0.5, torch.ones_like(vt[:, 0])], dim=-1)
-        p2f, bary, _ = ops.raster_mesh(uv[None], ft, R, R)
+        p2f, bary = uv_raster(vt, ft, R, R)
         p2f, bary = p2f.view(R * R), bary.view(R * R, 3)
         self.tex_mask = (p2f >= 0).view(R, R)
         self.texel_index = torch.nonzero(p2f >= 0).view(-1)
